@@ -52,16 +52,20 @@ __device__ __forceinline__ void spmm_row(const SpmmArgs<T>& a, int row, int lane
 #pragma unroll
             for (int u = 0; u < 4; u++) {
                 kk[u] = __shfl_sync(0xffffffffu, c, (t + u) & 31);
-                vv[u] = __shfl_sync(0xffffffffu, v, (t + u) & 31);   // lanes beyond cnt carry v = 0, c = 0: harmless
+                vv[u] = __shfl_sync(0xffffffffu, v, (t + u) & 31);
             }
+            // t + u >= cnt: no entry (the shuffled column is 0), so neither a load nor a product -- an Inf or NaN in row 0
+            // of B must not reach rows that do not store column 0.  cnt and t are warp-uniform: no divergence.
 #pragma unroll
             for (int u = 0; u < 4; u++) {
                 const long long ro = (long long)kk[u] * a.sbk;
-                b0[u] = la ? __ldg(Ba + ro) : T(0);
-                b1[u] = lb ? __ldg(Bb + ro) : T(0);
+                const bool live = t + u < cnt;
+                b0[u] = la && live ? __ldg(Ba + ro) : T(0);
+                b1[u] = lb && live ? __ldg(Bb + ro) : T(0);
             }
 #pragma unroll
-            for (int u = 0; u < 4; u++) { acc0 += vv[u] * b0[u]; acc1 += vv[u] * b1[u]; }
+            for (int u = 0; u < 4; u++)
+                if (t + u < cnt) { acc0 += vv[u] * b0[u]; acc1 += vv[u] * b1[u]; }
         }
     }
 }

@@ -299,6 +299,7 @@ __device__ __forceinline__ void sell_issue(const SellArgs<T>& a, int row, SellRo
         const bool live = u < r.width;
         r.c[u] = live ? ldg_stream(a.col + r.first + (size_t)u * C) - a.base : -1;
         r.v[u] = live ? ldg_stream(a.val + r.first + (size_t)u * C) : T(0);
+        if (r.c[u] < 0) r.v[u] = T(0);        // padding: its stored value takes no part (NaN there must not reach y)
     }
 }
 
@@ -330,6 +331,7 @@ __global__ void __launch_bounds__(SELL_BLOCK, sizeof(T) == 4 ? B200_SELL_MIN_CTA
                 const bool live = k + u < cur.width;
                 cc[u] = live ? ldg_stream(a.col + cur.first + (size_t)(k + u) * C) - a.base : -1;
                 vv[u] = live ? ldg_stream(a.val + cur.first + (size_t)(k + u) * C) : T(0);
+                if (cc[u] < 0) vv[u] = T(0);      // padding
             }
 #pragma unroll
             for (int u = 0; u < SELL_UNROLL; u++) xv[u] = cc[u] >= 0 ? __ldg(a.x + cc[u]) : T(0);
@@ -355,7 +357,10 @@ __device__ __forceinline__ T sell32_row(const int* __restrict__ cp, const T* __r
 #pragma unroll
     for (int u = 0; u < W; u++) { c[u] = ldg_stream(cp + u * 32); v[u] = ldg_stream(vp + u * 32); }
 #pragma unroll
-    for (int u = 0; u < W; u++) x[u] = c[u] >= base ? __ldg(xp + c[u]) : T(0);     // padding: column -1 (+base)
+    for (int u = 0; u < W; u++) {                       // padding: column -1 (+base); neither x nor the stored value is used
+        x[u] = c[u] >= base ? __ldg(xp + c[u]) : T(0);
+        v[u] = c[u] >= base ? v[u] : T(0);
+    }
     T sum = v[0] * x[0];
 #pragma unroll
     for (int u = 1; u < W; u++) sum += v[u] * x[u];

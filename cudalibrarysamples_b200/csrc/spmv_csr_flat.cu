@@ -517,6 +517,12 @@ void b200spmv_csr_flat_plan_offsets(int64_t rows, int64_t nnz, size_t* endmask, 
     if (ctl) *ctl = (size_t)((char*)p.ctl - (char*)nullptr);
 }
 
+void b200spmv_csr_flat_params(int32_t* warp_chunk, int32_t* cta_nnz, int32_t* plan_chunk) {
+    if (warp_chunk) *warp_chunk = FLAT_CHUNK;
+    if (cta_nnz) *cta_nnz = FLAT_CTA_NNZ;
+    if (plan_chunk) *plan_chunk = PLAN_CHUNK;
+}
+
 int b200spmv_csr_flat_mv(void* stream, int dtype, int64_t rows, int64_t cols, int64_t nnz, const void* row_offsets,
                          const void* col_ind, const void* values, int32_t base, const void* alpha, const void* beta,
                          int scalars_on_device, const void* x, void* y, void* workspace) {

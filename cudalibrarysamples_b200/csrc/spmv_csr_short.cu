@@ -167,6 +167,11 @@ extern "C" {
 
 int b200spmv_csr_short_max_row(void) { return SHORT_MAX_ROW; }
 
+void b200spmv_csr_short_params(int32_t* pass_cap, int32_t* rows_per_warp) {
+    if (pass_cap) *pass_cap = SHORT_CAP;
+    if (rows_per_warp) *rows_per_warp = 32;
+}
+
 int b200spmv_csr_max_row_length(void* stream, int64_t rows, const void* row_offsets, int32_t* out_device) {
     if (rows < 0 || !out_device || (rows > 0 && !row_offsets)) return -1;
     cudaStream_t st = (cudaStream_t)stream;

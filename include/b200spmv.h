@@ -74,12 +74,17 @@ B200SPMV_EXPORT int    b200spmv_csr_flat_mv(void* stream, int dtype, int64_t row
  * {non-empty rows, steps without a row end, steps} -- read back by the bit-exact preprocessing tests */
 B200SPMV_EXPORT void   b200spmv_csr_flat_plan_offsets(int64_t rows, int64_t nnz, size_t* endmask, size_t* chunk_run,
                                                       size_t* nzrow, size_t* ctl);
+/* the constants csr_flat_kernel was built with: non-zeros per warp chunk, per CTA, and per chunk_run entry of the plan
+ * (the exact-arithmetic tests place row ends around these borders) */
+B200SPMV_EXPORT void   b200spmv_csr_flat_params(int32_t* warp_chunk, int32_t* cta_nnz, int32_t* plan_chunk);
 
 /* CSR, all rows short (spmv_csr_short.cu): a warp per 32 consecutive rows, products staged in the warp's own slice of
  * shared memory, one lane per row adds them up; needs no plan, only the caller's row offsets.  cusparseSpMV_preprocess picks
  * it when the longest row (b200spmv_csr_max_row_length, written to device memory) has at most b200spmv_csr_short_max_row()
  * non-zeros -- the stencil operators of cuSPARSE/cg/cg_example.c:71-128 and cuSPARSE/bicgstab/bicgstab_example.c:69-127. */
 B200SPMV_EXPORT int    b200spmv_csr_short_max_row(void);
+/* csr_short_kernel's constants: products one warp stages per pass (SHORT_CAP), rows per warp */
+B200SPMV_EXPORT void   b200spmv_csr_short_params(int32_t* pass_cap, int32_t* rows_per_warp);
 B200SPMV_EXPORT int    b200spmv_csr_max_row_length(void* stream, int64_t rows, const void* row_offsets, int32_t* out_device);
 B200SPMV_EXPORT int    b200spmv_csr_short_mv(void* stream, int dtype, int64_t rows, int64_t cols, int64_t nnz,
                                              const void* row_offsets, const void* col_ind, const void* values,

@@ -230,3 +230,43 @@ def test_sell_index_widths_and_transposes(cs, b200, closed, off_bits, col_bits, 
     arrays = dict(off=dev(so.astype(NPI[off_bits])), col=dev(sc.astype(NPI[col_bits])), val=dev(sv), slice_size=slice_size,
                   nnz=int(col.size))
     check(cs, b200, closed, "sell", rows, cols, arrays, (off, col, va), base, transpose, types)
+
+
+# ------------------------------------------------------------------------------------------ exact fixtures (oracle/exact.py)
+@pytest.mark.parametrize("kind", ["f32", "f64", "wide", "mixed"])
+@pytest.mark.parametrize("transpose", [False, True])
+def test_coo_and_sell_generic_exact(cs, b200, kind, transpose):
+    """coo_generic_kernel (64-bit indices) and sell_generic_kernel (A and A^T) on the exact fixtures: bit-equal to the int64
+    reference, beta = 0 on a NaN-filled y included."""
+    from oracle import exact as E
+    lens = np.concatenate([[0, 3, 1, 0, 0, 40], np.full(70, 5), [600, 0, 1] * 5, [0, 0]])
+    f = E.Fixture("mix", lens, 900, kind, seed=4)
+    xy = torch.float64 if E.NP_XY[kind] == np.float64 else torch.float32
+    row = np.repeat(np.arange(f.rows, dtype=np.int64), np.diff(f.off))
+    coo = dict(row=dev(row), col=dev(f.col.astype(np.int64)), val=dev(f.val))
+    so, sc, sv = E.to_sell(f.off, f.col, f.val, 7)
+    sell = dict(off=dev(so.astype(np.int64)), col=dev(sc.astype(np.int64)), val=dev(sv), slice_size=7, nnz=f.nnz)
+    for fmt, arrays in (("coo", coo), ("sell", sell)):
+        for alpha, beta in E.SCALARS:
+            y0 = f.y0f(transpose)
+            y = torch.full((y0.size,), float("nan"), dtype=xy, device="cuda") if beta == 0 else dev(y0).to(xy)
+            got = spmv(cs, b200, fmt, f.rows, f.cols, arrays, dev(f.xf(transpose)).to(xy), y, alpha, beta, 0, transpose, xy).cpu().numpy()
+            assert np.array_equal(got.astype(np.float64), f.want(alpha, beta, transpose=transpose)), (fmt, alpha, beta)
+
+
+@pytest.mark.parametrize("kind", ["f32", "f64"])
+def test_batched_spmm_exact(cs, b200, kind):
+    """strided-batch SpMM, three matrices sharing row offsets, on exact integer data: bit-equal to the int64 reference"""
+    from oracle import exact as E
+    rows, n, batches = 300, 33, 3
+    f = E.Fixture("b", np.full(rows, 6), rows, kind, seed=6)
+    npdt = E.NP_A[kind]
+    vals = [E.values(kind, f.nnz, 0, 0, 40 + i)[0] for i in range(batches)]
+    Bs = [E.values(kind, 0, rows * n, 0, 50 + i)[1].reshape(rows, n) for i in range(batches)]
+    C0s = [E.values(kind, 0, 0, rows * n, 60 + i)[2].reshape(rows, n) for i in range(batches)]
+    got = native(b200, lambda: cs.spmm_batched(b200, rows, rows, f.nnz, batches, dev(f.off), dev(np.tile(f.col, batches)),
+                                               dev(np.concatenate(vals).astype(npdt)), dev(np.concatenate(Bs).astype(npdt).reshape(-1)),
+                                               dev(np.concatenate(C0s).astype(npdt).reshape(-1)), -2.0, 0.5, order=2)).cpu().numpy()
+    for i in range(batches):
+        want = E.spmm_reference(f.off, f.col, vals[i], Bs[i], C0s[i], -2.0, 0.5)
+        assert np.array_equal(got[rows * n * i:rows * n * (i + 1)].reshape(rows, n).astype(np.float64), want), i
