@@ -73,7 +73,7 @@ class CgSolver:
 
 
 class FusedCgSolver:
-    """The same iteration on the fused sm_90a BLAS-1 kernels of csrc/cg_fused.cu (b200cg_dot / _update_xr / _update_p): per
+    """The same iteration on the fused sm_90a BLAS-1 kernels of csrc/cg_fused.cu (b200cg_dot / _update_r / _update_xp): per
     iteration 1 SpMV + 3 kernels, every scalar in device memory, partial dots all-reduced over ranks; on one GPU two
     iterations are captured in a CUDA graph and replayed (graph_capture_example.c:118-135 pattern)."""
 
@@ -121,7 +121,7 @@ class FusedCgSolver:
             self.sh.spmv(p, t, alpha=1.0, beta=0.0)                          # T = A * P      (cg_example.c:220-224)
             self._dot(t, p, s[2:3])                                          # denom = T . P  (:227)
         nxt = 1 - cur
-        # 8 vector passes: R -= aT with delta' = R.R, then X += aP and P = R + (delta'/delta) P in one pass (P read once)
+        # 8 vector passes after the dot's 2: R -= aT with delta' = R.R, then X += aP and P = R + (delta'/delta) P in one pass (P read once)
         self._check(self.L.b200cg_update_r(self._stream(), C.c_int64(self.n), self._p(r), self._p(t), self._p(s[cur:cur + 1]), self._p(s[2:3]),
                                            self._p(s[nxt:nxt + 1]), self._p(self.ws)), "b200cg_update_r")       # (:241-247)
         if self.sh.world > 1:
@@ -185,7 +185,7 @@ class FusedCgSolver:
         spmv = ("T = A*P and T.P in one csr_short_kernel launch (b200spmv_csr_short_mv_dot)" if self.fuse_dot
                 else "SpMV through the C ABI + b200cg_dot")
         return ("CG (cg_example.c:215-287 without the IC(0) preconditioner): " + spmv + " + fused sm_90a BLAS-1 kernels "
-                "(b200cg_update_r = axpy + nrm2 in one pass, b200cg_update_xp = x and p updates in one pass: 8 vector passes per iteration), all scalars on the device, "
+                "(b200cg_update_r = axpy + nrm2 in one pass, b200cg_update_xp = x and p updates in one pass: 10 vector passes per iteration with the dot), all scalars on the device, "
                 + how + (f" (graph capture failed: {self.graph_error})" if self.graph_error else ""))
 
 

@@ -7,7 +7,8 @@
 //     cublasDnrm2(R) -> host            (:247)      /
 //     beta = delta_new / delta on host  (:280)      \
 //     cublasDscal + cublasDaxpy on P    (:281-286)  /   b200cg_update_p    one pass: p = r + beta * p
-// ... or, one vector pass cheaper (8 instead of 9 per iteration: p is read once, next to its own update):
+// ... or, one vector pass cheaper (10 instead of 11 per iteration, counting every whole-vector read and write including the
+// 2 of b200cg_dot: p is read once, next to its own update):
 //     b200cg_update_r   r -= alpha t, r.r in the same pass        b200cg_update_xp   x += alpha p_old;  p = r + beta p_old
 // No host synchronisation anywhere: scalars are read from / written to device memory, so the whole iteration can be
 // captured in a CUDA graph (cuSPARSE/graph_capture/graph_capture_example.c:118-135 shows the pattern for SpVV).
@@ -114,7 +115,7 @@ __global__ void __launch_bounds__(BLOCK) update_p_kernel(int64_t n, double* __re
     }
 }
 
-// --- the same iteration in 8 instead of 9 vector passes: the x update moves next to the p update (p is read once) ---
+// --- the same iteration in 10 instead of 11 vector passes (dot included): the x update moves next to the p update (p is read once) ---
 // alpha = delta / denom;  r -= alpha t;  delta_new = r . r          (reads t, r; writes r)
 __global__ void __launch_bounds__(BLOCK) update_r_kernel(int64_t n, double* __restrict__ r, const double* __restrict__ t,
                                                          const double* __restrict__ delta, const double* __restrict__ denom,
@@ -176,6 +177,11 @@ using namespace b200cg;
 extern "C" {
 
 size_t b200cg_workspace_bytes(void) { return (MAX_CTAS + 2) * sizeof(double); }
+
+void b200cg_params(int32_t* block, int32_t* max_ctas) {
+    if (block) *block = BLOCK;
+    if (max_ctas) *max_ctas = MAX_CTAS;
+}
 
 // the workspace must be zeroed once (cudaMemset) before its first use; every call leaves the arrival counter at zero
 int b200cg_dot(void* stream, int64_t n, const double* a, const double* b, double* out, void* workspace) {

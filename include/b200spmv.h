@@ -128,13 +128,20 @@ B200SPMV_EXPORT int b200spmm_csr(void* stream, int dtype, int64_t rows, int64_t 
  * once by the caller.
  *   b200cg_dot        *out = a . b
  *   b200cg_update_xr  alpha = *delta / *denom;  x += alpha p;  r -= alpha t;  *delta_new = r . r   (one pass)
- *   b200cg_update_p   beta = *delta_new / *delta;  p = r + beta p */
+ *   b200cg_update_p   beta = *delta_new / *delta;  p = r + beta p
+ * Every kernel walks the vectors in pairs (16-byte loads, a scalar tail for odd n) with a grid-stride loop over
+ * min(ceil((n / 2) / block), max_ctas) CTAs of `block` threads; the workspace holds max_ctas partial sums, then the arrival
+ * counter (uint32 at byte max_ctas * 8), which every reduction leaves at zero.  b200cg_params reports block and max_ctas
+ * (the exact-arithmetic tests size their vectors around these borders). */
 B200SPMV_EXPORT size_t b200cg_workspace_bytes(void);
+B200SPMV_EXPORT void   b200cg_params(int32_t* block, int32_t* max_ctas);
 B200SPMV_EXPORT int    b200cg_dot(void* stream, int64_t n, const double* a, const double* b, double* out, void* workspace);
 B200SPMV_EXPORT int    b200cg_update_xr(void* stream, int64_t n, double* x, double* r, const double* p, const double* t,
                                         const double* delta, const double* denom, double* delta_new, void* workspace);
 /*   b200cg_update_r   alpha = *delta / *denom;  r -= alpha t;  *delta_new = r . r            (x is not touched)
- *   b200cg_update_xp  x += alpha p;  beta = *delta_new / *delta;  p = r + beta p              (p read once: 8 vector passes per iteration instead of 9) */
+ *   b200cg_update_xp  x += alpha p;  beta = *delta_new / *delta;  p = r + beta p              (p read once)
+ * A CG iteration of b200cg_dot + _update_r + _update_xp reads or writes a whole vector 10 times (2 + 3 + 5); with _update_xr +
+ * _update_p instead it is 11 (2 + 6 + 3). */
 B200SPMV_EXPORT int    b200cg_update_r(void* stream, int64_t n, double* r, const double* t, const double* delta, const double* denom,
                                        double* delta_new, void* workspace);
 B200SPMV_EXPORT int    b200cg_update_xp(void* stream, int64_t n, double* x, double* p, const double* r, const double* delta,

@@ -16,10 +16,15 @@ sum |products| and 2 * (|alpha| * sum |products| + |beta * y0|) stay below 2^p (
 
 The boundary profiles are row-length sequences built from the kernels' own constants (read from the built library by
 `kernel_params`), and `coverage` recomputes from the row offsets which boundary class a matrix actually hits.
+
+The fused CG BLAS-1 kernels (cg_fused.cu) get the same treatment at the end of this file: vectors of nonzero integers, device
+scalars whose quotients are powers of two (alpha = -1/4, beta = 1/2), an int64 reference on values scaled by 4 (vectors) and
+16 (r . r), edge sizes built from `cg_params`, and `cg_walk` / `cg_coverage`, a model of the kernels' index mapping.
 """
 from __future__ import annotations
 
 import ctypes as C
+from fractions import Fraction
 
 import numpy as np
 
@@ -354,3 +359,156 @@ def coverage(off, cols, P: dict) -> set:
         if np.any(tot == t):
             hit.add(f"short_block_{name}")
     return hit
+
+
+# ------------------------------------------------------------------------------------------------ fused CG BLAS-1 (cg_fused.cu)
+def cg_params(lib=None) -> dict:
+    """block (threads per CTA) and max_ctas (grid cap) of the built library's CG kernels (b200cg_params)"""
+    if lib is None:
+        from cudalibrarysamples_b200 import lib as _lib
+        lib = _lib.shim()
+    b, m = C.c_int32(), C.c_int32()
+    lib.b200cg_params(C.byref(b), C.byref(m))
+    return dict(block=b.value, max_ctas=m.value)
+
+
+def cg_grid(n, P):
+    """CTAs of a launch over n elements (grid_for in cg_fused.cu: one pair per thread, capped)"""
+    g = (n // 2 + P["block"] - 1) // P["block"]
+    return int(max(1, min(g, P["max_ctas"])))
+
+
+def cg_walk(n, P):
+    """The index walk every kernel of cg_fused.cu makes: thread k of the grid starts at pair index 2k and strides by
+    2 * grid * block; i + 1 < n takes the 16-byte path (elements i, i + 1), otherwise the scalar path (element i).
+    Returns grid, passes (grid-stride trips of thread 0), visits[i] (how often element i is read) and the trip on which the
+    scalar path ran (None if it never did)."""
+    g = cg_grid(n, P)
+    first = 2 * np.arange(g * P["block"], dtype=np.int64)
+    stride = 2 * g * P["block"]
+    visits = np.zeros(n, np.int64)
+    passes, scalar_pass, scalar_visits = 0, None, 0
+    while True:
+        i = first + passes * stride
+        i = i[i < n]
+        if i.size == 0:
+            break
+        pair, single = i[i + 1 < n], i[i + 1 >= n]
+        visits[pair] += 1
+        visits[pair + 1] += 1
+        visits[single] += 1
+        if single.size:
+            scalar_pass, scalar_visits = passes, scalar_visits + single.size
+        passes += 1
+    return dict(grid=g, passes=passes, visits=visits, scalar_pass=scalar_pass, scalar_visits=scalar_visits)
+
+
+def cg_full_pass(P):
+    """F: elements one grid-stride pass covers at the grid cap"""
+    return P["max_ctas"] * 2 * P["block"]
+
+
+def cg_sizes(P):
+    """Vector lengths around the kernels' borders: P2 = 2 * block elements per CTA pass, F per full-grid pass"""
+    P2, F = 2 * P["block"], cg_full_pass(P)
+    first_at_cap = 2 * ((P["max_ctas"] - 1) * P["block"] + 1)          # smallest n with cg_grid(n) == max_ctas
+    return [0, 1, 2, 3, 33, P2 - 1, P2, P2 + 1, 2 * P2 + 1, 5 * P2 + 1, first_at_cap, F - 1, F, F + 1, F + 2, 2 * F, 2 * F + 3,
+            3 * F + P2 + 1]
+
+
+CG_CLASSES = ["n_zero", "scalar_tail_only", "odd_tail_first_pass", "odd_tail_later_pass_below_cap", "odd_tail_later_pass_at_cap",
+              "one_cta", "two_ctas", "cap_single_pass", "exactly_one_full_pass", "multi_pass_partial_last",
+              "multi_pass_whole_passes"]
+
+
+def cg_coverage(n, P) -> set:
+    """Which of CG_CLASSES a launch over n elements falls in, from the index model"""
+    w = cg_walk(n, P)
+    F, cap = cg_full_pass(P), w["grid"] == P["max_ctas"]
+    sp = w["scalar_pass"]
+    hit = set()
+    if n == 0:
+        return {"n_zero"}
+    if n == 1:
+        hit.add("scalar_tail_only")
+    elif sp == 0:
+        hit.add("odd_tail_first_pass")
+    if sp is not None and sp > 0:
+        hit.add("odd_tail_later_pass_at_cap" if cap else "odd_tail_later_pass_below_cap")
+    if w["grid"] in (1, 2):
+        hit.add("one_cta" if w["grid"] == 1 else "two_ctas")
+    if cap and w["passes"] == 1:
+        hit.add("cap_single_pass")
+    if n == F:
+        hit.add("exactly_one_full_pass")
+    if w["passes"] > 1 and cap:
+        hit.add("multi_pass_whole_passes" if n % F == 0 else "multi_pass_partial_last")
+    return hit
+
+
+CG_KINDS = ["f64", "wide"]
+_CG_RANGES = {"f64": (1, 5), "wide": (1 << 12, 1 << 13)}      # |value|: products of "wide" need 25-26 bits, sums far more than fp32 has
+# the device scalars: alpha = delta / denom = -1/4 and beta = delta_new / delta = 1/2, both exact divisions
+CG_SCALARS = dict(delta=3.0, denom=-12.0, delta_new=1.5)
+
+
+class CgKernel:
+    """One entry point: its vector arguments and device-scalar arguments in call order (the workspace comes last when
+    `workspace`), the vectors it writes and the scalar it reduces into (None: no reduction)."""
+
+    def __init__(self, vectors, scalars, writes, reduces, workspace):
+        self.vectors, self.scalars, self.writes, self.reduces, self.workspace = vectors, scalars, writes, reduces, workspace
+
+
+CG_KERNELS = {
+    "dot": CgKernel(["a", "b"], ["out"], [], "out", True),
+    "update_r": CgKernel(["r", "t"], ["delta", "denom", "delta_new"], ["r"], "delta_new", True),
+    "update_xr": CgKernel(["x", "r", "p", "t"], ["delta", "denom", "delta_new"], ["x", "r"], "delta_new", True),
+    "update_xp": CgKernel(["x", "p", "r"], ["delta", "denom", "delta_new"], ["x", "p"], None, False),
+    "update_p": CgKernel(["p", "r"], ["delta_new", "delta"], ["p"], None, False),
+}
+
+
+def cg_vectors(kind, n, names, seed):
+    """int64 vectors of n nonzero integers each (|v| in the kind's range), one per name"""
+    rng = np.random.default_rng(seed)
+    lo, hi = _CG_RANGES[kind]
+    return {k: nonzero_ints(rng, n, lo, hi) for k in names}
+
+
+def _dyadic(q: Fraction):
+    assert q.denominator & (q.denominator - 1) == 0, f"{q}: not a dyadic quotient"
+    return q.numerator, q.denominator
+
+
+def _exact_float(num, den):
+    """num / den as float64, asserting that it is exact (|num| < 2^53, den a power of two)"""
+    assert np.all(np.abs(num) < (1 << 53)), "a result needs more than 53 bits"
+    return np.asarray(num, np.int64).astype(np.float64) / den
+
+
+def cg_reference(name, v, scal=CG_SCALARS):
+    """What kernel `name` must produce from the int64 vectors v (dict) and the device scalars: {written vector or reduced
+    scalar: float64}, computed in integers.  Asserts the exactness precondition: every updated element is num / 4 with
+    |num| < 2^53, and the sum of |terms| of each reduction stays below 2^53 in units of its last place (1 for a . b, 1/16 for
+    r . r), so every partial sum in any order is exact."""
+    alpha = Fraction(scal["delta"]) / Fraction(scal["denom"])
+    beta = Fraction(scal["delta_new"]) / Fraction(scal["delta"])
+    an, ad = _dyadic(alpha)
+    bn, bd = _dyadic(beta)
+    out = {}
+    if name == "dot":
+        terms = v["a"] * v["b"]
+        assert int(np.abs(terms).sum()) < (1 << 53)
+        out["out"] = float(int(terms.sum()))
+    if name in ("update_r", "update_xr"):
+        rn = v["r"] * ad - an * v["t"]                       # r - alpha t, scaled by ad
+        sq = rn * rn
+        assert int(sq.sum()) < (1 << 53)
+        out["r"] = _exact_float(rn, ad)
+        out["delta_new"] = float(int(sq.sum())) / (ad * ad)
+    if name in ("update_xr", "update_xp"):
+        out["x"] = _exact_float(v["x"] * ad + an * v["p"], ad)      # x + alpha p
+    if name in ("update_xp", "update_p"):
+        out["p"] = _exact_float(v["r"] * bd + bn * v["p"], bd)      # r + beta p
+    return out

@@ -79,6 +79,12 @@ def test_library_loads_without_a_gpu(built_lib):
     assert nt == (17000 + t.value - 1) // t.value
     ws = lib.b200spmv_csr_workspace_bytes(ctypes.c_int64(1000), ctypes.c_int64(16000))
     assert ws >= (nt + 1) * (8 + 4 + 8 + 8)
+    # the CG workspace: one partial sum per CTA of the largest grid, then the arrival counter in its own 8-byte slot (+ 1 spare)
+    blk, max_ctas = ctypes.c_int32(), ctypes.c_int32()
+    lib.b200cg_params(ctypes.byref(blk), ctypes.byref(max_ctas))
+    assert blk.value % 32 == 0 and max_ctas.value > 0
+    lib.b200cg_workspace_bytes.restype = ctypes.c_size_t
+    assert lib.b200cg_workspace_bytes() == (max_ctas.value + 2) * 8
     # argument validation happens on the host, before any CUDA call
     assert lib.b200spmv_csr_mv(None, 7, ctypes.c_int64(4), ctypes.c_int64(4), ctypes.c_int64(9), None, None, None, 0,
                                None, None, 0, None, None, None) == -1

@@ -7,6 +7,7 @@ retuned constant that moves a border shows up), and that the numpy lane emulatio
 csr_short_kernel and the host-compiled source of the generic kernels reproduce the reference with np.array_equal.  The
 same fixtures run on the GPU in tests/test_exact_gpu.py."""
 import ctypes as C
+import math
 
 import numpy as np
 import pytest
@@ -203,3 +204,76 @@ def test_generic_sources_are_exact(emu, profiles, kind, base):
                     assert emu.emu_sell_generic(1, 1, a_dt, xy_dt, transpose, 1, LL(f.rows), LL(f.cols), LL(S), _p(so.astype(np.int64)),
                                                 _p(sc.astype(np.int64)), _p(sv), LL(base), C.byref(ca), C.byref(cb), _p(xf), _p(y)) == 0
                     assert np.array_equal(y, want), ("sell", name, transpose, S, alpha, beta)
+
+
+# ------------------------------------------------------------------------------------------ fused CG BLAS-1 (cg_fused.cu)
+@pytest.fixture(scope="module")
+def CGP(built_lib):
+    return E.cg_params()
+
+
+def test_cg_index_model_visits_every_element_once(CGP):
+    """The model of the kernels' index mapping: every index in [0, n) is read exactly once (one 16-byte pair or the scalar
+    tail), the scalar path runs at most once and only for odd n, and the grid never exceeds the cap."""
+    for n in E.cg_sizes(CGP):
+        w = E.cg_walk(n, CGP)
+        assert np.array_equal(w["visits"], np.ones(n, np.int64)), n
+        assert w["scalar_visits"] == n % 2, n
+        assert 1 <= w["grid"] <= CGP["max_ctas"]
+        assert w["passes"] == -(-n // (2 * w["grid"] * CGP["block"])), n
+
+
+def test_cg_sizes_cover_every_class(CGP):
+    hit = {}
+    for n in E.cg_sizes(CGP):
+        for c in E.cg_coverage(n, CGP):
+            hit.setdefault(c, []).append(n)
+    assert not set(E.CG_CLASSES) - set(hit), f"no size hits {sorted(set(E.CG_CLASSES) - set(hit))}"
+    F = E.cg_full_pass(CGP)
+    # the sizes sit on the kernels' borders: the first size at the grid cap, F itself, F + 1
+    first_at_cap = min(hit["cap_single_pass"])
+    assert E.cg_grid(first_at_cap, CGP) == CGP["max_ctas"] and E.cg_grid(first_at_cap - 2, CGP) == CGP["max_ctas"] - 1
+    assert hit["exactly_one_full_pass"] == [F] and F + 1 in hit["odd_tail_later_pass_at_cap"]
+    assert max(E.cg_walk(n, CGP)["passes"] for n in E.cg_sizes(CGP)) >= 4
+
+
+def test_cg_coverage_notices_a_missing_class(CGP):
+    """Without the sizes that carry them, classes go missing: the coverage check is not vacuous."""
+    P2, F = 2 * CGP["block"], E.cg_full_pass(CGP)
+    hit = set()
+    for n in E.cg_sizes(CGP):
+        if n not in (1, P2 + 1, 2 * P2 + 1, 5 * P2 + 1, F):
+            hit |= E.cg_coverage(n, CGP)
+    assert {"scalar_tail_only", "odd_tail_later_pass_below_cap", "exactly_one_full_pass"} <= set(E.CG_CLASSES) - hit
+
+
+@pytest.mark.parametrize("kind", E.CG_KINDS)
+def test_cg_reference_is_exact_at_every_size(CGP, kind):
+    """The precondition (asserted inside cg_reference) holds at every size up to the largest, and the reference agrees with
+    float64 numpy on the operations where float64 is exact too."""
+    for name, k in E.CG_KERNELS.items():
+        for n in E.cg_sizes(CGP):
+            v = E.cg_vectors(kind, n, k.vectors, seed=n)
+            want = E.cg_reference(name, v)
+            assert set(want) == set(k.writes) | ({k.reduces} if k.reduces else set())
+            f = {key: a.astype(np.float64) for key, a in v.items()}
+            if "x" in want:
+                assert np.array_equal(want["x"], f["x"] + (-0.25) * f["p"])
+            if "p" in want:
+                assert np.array_equal(want["p"], f["r"] + 0.5 * f["p"])
+            if "r" in want:
+                assert np.array_equal(want["r"], f["r"] - (-0.25) * f["t"])
+                assert want["delta_new"] == math.fsum(want["r"] * want["r"])
+            if name == "dot":
+                assert want["out"] == math.fsum(f["a"] * f["b"])
+
+
+def test_cg_wide_vectors_need_more_than_fp32(CGP):
+    """At the largest size an fp32 accumulator loses bits on both kinds; the "wide" products alone need more than 24 bits."""
+    n = E.cg_sizes(CGP)[-1]
+    for kind in E.CG_KINDS:
+        v = E.cg_vectors(kind, n, ["a", "b"], seed=1)
+        assert np.abs(v["a"] * v["b"]).sum() > 1 << 24
+    v = E.cg_vectors("wide", 1000, ["a", "b"], seed=1)
+    assert np.abs(v["a"] * v["b"]).min() >= 1 << 24
+    assert np.all(v["a"] != 0) and np.all(E.cg_vectors("f64", 1000, ["a"], seed=2)["a"] != 0)

@@ -98,6 +98,38 @@ def test_config4_poisson_8192_fp64_csr(env):
     assert float((interior - 0.75 * 0.04).abs().max().item()) < 1e-13
 
 
+def test_config4_cg_fused_driver_matches_torch_ops(env):
+    """BASELINE.json configs[3]'s CG at the size bench.py times (n = 8192^2: about 62 grid-stride passes of the fused BLAS-1
+    kernels at their grid cap): 20 iterations of the fused driver (CUDA graph on) against the torch-op driver on the same
+    operator, and the fused driver's recurrence norm against the true residual ||b - A x||."""
+    from cudalibrarysamples_b200.cg import CgSolver, FusedCgSolver
+    from cudalibrarysamples_b200.sharded import ShardedCsr
+    cs, W, ours, closed = env
+    g, iters = 8192, 20
+    n = g * g
+    off, col, val = W.stencil5_csr(g)
+
+    def make_local(r, c, arrays):
+        return cs.SpMVOperator(ours, "csr", r, c, arrays, preprocess=True)
+    sh = ShardedCsr(off, col, val, 0, 1, make_local, balance="rows")
+    del off, col, val
+    b = sh.new_y_shard()
+    sh.spmv(sh.new_x_shard(torch.ones(n, dtype=torch.float64, device="cuda")), b, alpha=0.75, beta=0.0)
+    fused = FusedCgSolver(sh, b, use_graph=True)
+    xf, nf = fused.run(iters)
+    torch.cuda.synchronize()
+    assert fused.graph_error is None, fused.graph_error
+    xt, nt = CgSolver(sh, b).run(iters)
+    assert abs(nf[0] - nt[0]) <= 1e-9 * nt[0] and abs(nf[-1] - nt[-1]) <= 1e-9 * nt[-1], (nf, nt[0], nt[-1])
+    assert rel(xf, xt) < 1e-9
+    del xt
+    res = b.clone()
+    sh.spmv(xf, res, alpha=-1.0, beta=1.0)                                  # b - A x
+    true = float(torch.linalg.norm(res).item())
+    assert true <= 1.01 * nf[-1] + 1e-12, (true, nf[-1])
+    sh.close()
+
+
 def test_north_star_rmat_10m_fp64_csr(env):
     """BASELINE.json north_star acceptance size: R-MAT 10,000,000 x 10,000,000, avg 16 nnz/row, fp64;
     ||y - y_ref|| / ||y_ref|| < 1e-12 against the closed library, through the preprocessed call sequence of

@@ -6,6 +6,7 @@ Tolerances (north_star): fp64 ||y - y_ref|| / ||y_ref|| < 1e-12, fp32 < 1e-5; in
 """
 import ctypes as C
 import json
+import math
 import os
 import subprocess
 
@@ -509,42 +510,87 @@ def test_sell_ragged_rmat(cs, b200):
 @pytest.mark.parametrize("graph", [False, True])
 def test_fused_cg_matches_the_sample_loop(cs, b200, graph, fuse_dot):
     """The fused device-scalar CG driver (csrc/cg_fused.cu) against a plain numpy restatement of cg_example.c:215-287
-    (no preconditioner) on the sample's own matrix family; with and without CUDA-graph replay."""
+    (no preconditioner) on the sample's own matrix family; with and without CUDA-graph replay.  Three grids: n = 96^2 is even
+    and fits one grid-stride pass; 97^2 is odd (the kernels' scalar tail); 1041^2 is odd and larger than one pass at the grid
+    cap."""
     from cudalibrarysamples_b200.cg import CgSolver, FusedCgSolver
     from cudalibrarysamples_b200.sharded import ShardedCsr
-    grid = 96
+    for grid in (96, 97, 1041):
+        off, col, val = O.gen_stencil5(grid)
+        n = grid * grid
+        b = O.spmv_csr(off, col, val, np.ones(n), alpha=0.75)            # cg_example.c:405-418
+        # reference loop on the CPU with the oracle SpMV
+        x = np.zeros(n); r = b.copy(); p = r.copy(); delta = r @ r
+        iters = 25
+        for _ in range(iters):
+            t = O.spmv_csr(off, col, val, p)
+            alpha = delta / (t @ p)
+            x += alpha * p; r -= alpha * t
+            dn = r @ r
+            p = r + (dn / delta) * p
+            delta = dn
+
+        def make_local(rr, cc, arrays):
+            return cs.SpMVOperator(b200, "csr", rr, cc, arrays, preprocess=True)
+        sh = ShardedCsr(dev(off), dev(col), dev(val), 0, 1, make_local, balance="rows")
+        solver = FusedCgSolver(sh, dev(b), use_graph=graph)
+        solver.fuse_dot = fuse_dot and sh.can_fuse_dot()          # T = A*P with T.P in its epilogue (opt-in: B200CG_FUSE_DOT=1)
+        assert solver.fuse_dot == fuse_dot, grid
+        xs, norms = solver.run(iters)
+        torch.cuda.synchronize()
+        assert solver.graph_error is None, (grid, solver.graph_error)
+        assert abs(norms[0] - np.sqrt(b @ b)) <= 1e-12 * np.sqrt(b @ b), grid
+        assert abs(norms[-1] - np.sqrt(delta)) <= 1e-6 * np.sqrt(delta), grid          # 25 iterations of rounding differences
+        assert relerr(xs.cpu().numpy(), x) < 1e-9, grid
+        # a second run on the same solver (bench: warm-up run, then the timed run) gives the same answer
+        xs2, norms2 = solver.run(iters)
+        assert torch.equal(xs, xs2) and norms2 == norms, grid
+        # and the torch-op driver agrees
+        xt, nt = CgSolver(sh, dev(b)).run(iters)
+        assert relerr(xt.cpu().numpy(), x) < 1e-9, grid
+        sh.close()
+
+
+@pytest.mark.parametrize("fuse_dot", [False, True])
+def test_fused_cg_graph_replay_gives_the_eager_bits(cs, b200, fuse_dot):
+    """FusedCgSolver.run with and without the CUDA graph gives bit-identical x and norms for every iteration count: below 4
+    (no graph), even and odd counts (the iterations left after the last replay run eagerly; the last delta sits in
+    scal[iters & 1]).  norms[0] is sqrt(b . b) of b200cg_dot, bit for bit."""
+    from cudalibrarysamples_b200 import lib as _lib
+    from cudalibrarysamples_b200.cg import FusedCgSolver
+    from cudalibrarysamples_b200.sharded import ShardedCsr
+    grid = 97
     off, col, val = O.gen_stencil5(grid)
     n = grid * grid
-    b = O.spmv_csr(off, col, val, np.ones(n), alpha=0.75)            # cg_example.c:405-418
-    # reference loop on the CPU with the oracle SpMV
-    x = np.zeros(n); r = b.copy(); p = r.copy(); delta = r @ r
-    iters = 25
-    for _ in range(iters):
-        t = O.spmv_csr(off, col, val, p)
-        alpha = delta / (t @ p)
-        x += alpha * p; r -= alpha * t
-        dn = r @ r
-        p = r + (dn / delta) * p
-        delta = dn
+    b = dev(O.spmv_csr(off, col, val, np.ones(n), alpha=0.75))
 
     def make_local(rr, cc, arrays):
         return cs.SpMVOperator(b200, "csr", rr, cc, arrays, preprocess=True)
     sh = ShardedCsr(dev(off), dev(col), dev(val), 0, 1, make_local, balance="rows")
-    solver = FusedCgSolver(sh, dev(b), use_graph=graph)
-    solver.fuse_dot = fuse_dot and sh.can_fuse_dot()          # T = A*P with T.P in its epilogue (opt-in: B200CG_FUSE_DOT=1)
-    assert solver.fuse_dot == fuse_dot
-    xs, norms = solver.run(iters)
-    torch.cuda.synchronize()
-    assert solver.graph_error is None, solver.graph_error
-    assert abs(norms[0] - np.sqrt(b @ b)) <= 1e-12 * np.sqrt(b @ b)
-    assert abs(norms[-1] - np.sqrt(delta)) <= 1e-6 * np.sqrt(delta)          # 25 iterations of rounding differences
-    assert relerr(xs.cpu().numpy(), x) < 1e-9
-    # a second run on the same solver (bench: warm-up run, then the timed run) gives the same answer
-    xs2, norms2 = solver.run(iters)
-    assert torch.equal(xs, xs2) and norms2 == norms
-    # and the torch-op driver agrees
-    xt, nt = CgSolver(sh, dev(b)).run(iters)
-    assert relerr(xt.cpu().numpy(), x) < 1e-9
+    L = _lib.shim()
+    L.b200cg_workspace_bytes.restype = C.c_size_t
+    ws = torch.zeros(int(L.b200cg_workspace_bytes()), dtype=torch.uint8, device="cuda")
+    bb = torch.full((1,), float("nan"), dtype=torch.float64, device="cuda")
+    assert L.b200cg_dot(C.c_void_p(torch.cuda.current_stream().cuda_stream), C.c_int64(n), C.c_void_p(b.data_ptr()),
+                        C.c_void_p(b.data_ptr()), C.c_void_p(bb.data_ptr()), C.c_void_p(ws.data_ptr())) == 0
+    norm0 = math.sqrt(float(bb.item()))
+    last = []
+    for iters in (0, 1, 2, 3, 4, 5, 6, 7, 10):
+        runs = {}
+        for graph in (False, True):
+            solver = FusedCgSolver(sh, b, use_graph=graph)
+            solver.fuse_dot = fuse_dot and sh.can_fuse_dot()
+            assert solver.fuse_dot == fuse_dot
+            x, norms = solver.run(iters)
+            torch.cuda.synchronize()
+            assert solver.graph_error is None, solver.graph_error
+            runs[graph] = (x.clone(), norms)
+        (xe, ne), (xg, ng) = runs[False], runs[True]
+        assert torch.equal(xe.view(torch.int64), xg.view(torch.int64)), f"iters={iters}: x differs between graph and eager"
+        assert ne == ng, f"iters={iters}: norms {ng} (graph) vs {ne} (eager)"
+        assert len(ne) == 2 and ne[0] == norm0, (iters, ne[0], norm0)
+        last.append(ne[1])
+    assert last[0] == norm0 and len(set(last)) == len(last), f"an iteration count repeated another's result: {last}"
     sh.close()
 
 
