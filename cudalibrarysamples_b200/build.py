@@ -2,6 +2,8 @@
 
   libb200spmv.so  the product: sm_90a kernels + the cuSPARSE-symbol shim (include/b200spmv.h)
   libb200gen.so   bench / test plumbing: synthetic-workload generators on the device (include/b200gen.h)
+  libb200spsv.so  the opt-in CSR triangular solve: sm_90a kernels + the cusparseSpSV_* shim (include/b200spsv.h); it does
+                  not link against libb200spmv.so
 
 The .so files are build products and git-ignored.  nvcc cross-compiles for sm_90a without a GPU, so this also runs
 on a machine that has none.
@@ -17,10 +19,12 @@ PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libb200spmv.so")
 GEN_LIB_PATH = os.path.join(PKG_DIR, "libb200gen.so")
-SOURCES = ["spmv_csr.cu", "spmv_csr_flat.cu", "spmv_csr_short.cu", "spmv_csr_transpose.cu", "spmv_coo_sell.cu", "spmv_generic.cu", "spmm_csr.cu", "cg_fused.cu", "peer_sync.cu", "config.cpp", "cusparse_shim.cpp"]
+SPSV_LIB_PATH = os.path.join(PKG_DIR, "libb200spsv.so")
+SOURCES = ["spmv_csr.cu", "spmv_csr_flat.cu", "spmv_csr_short.cu", "spmv_csr_transpose.cu", "spmv_coo_sell.cu", "spmv_generic.cu", "spmm_csr.cu", "cg_fused.cu", "peer_sync.cu", "config.cpp", "cusparse_shim.cpp", "real_cusparse.cpp"]
 GEN_SOURCES = ["workload_gen.cu"]
-HEADERS = ["spmv_common.cuh", "spmv_generic_kernels.cuh", "config.h", os.path.join("..", "..", "include", "b200spmv.h"),
-           os.path.join("..", "..", "include", "b200gen.h")]
+SPSV_SOURCES = ["spsv_csr.cu", "spsv_shim.cpp", "real_cusparse.cpp"]
+HEADERS = ["spmv_common.cuh", "spmv_generic_kernels.cuh", "config.h", "real_cusparse.h", os.path.join("..", "..", "include", "b200spmv.h"),
+           os.path.join("..", "..", "include", "b200gen.h"), os.path.join("..", "..", "include", "b200spsv.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -46,7 +50,7 @@ def _stale(target: str, sources) -> bool:
 
 
 def needs_build() -> bool:
-    return _stale(LIB_PATH, SOURCES) or _stale(GEN_LIB_PATH, GEN_SOURCES)
+    return _stale(LIB_PATH, SOURCES) or _stale(GEN_LIB_PATH, GEN_SOURCES) or _stale(SPSV_LIB_PATH, SPSV_SOURCES)
 
 
 def _compile_and_link(sources, target, build_dir, extra_flags, log):
@@ -77,7 +81,7 @@ def _compile_and_link(sources, target, build_dir, extra_flags, log):
 
 def build_native(force: bool = False, verbose: bool = False, extra_flags=(), out_path: str | None = None,
                  tag: str = "") -> str:
-    """Compile every CUDA source for sm_90a into cudalibrarysamples_b200/libb200spmv.so (+ libb200gen.so).
+    """Compile every CUDA source for sm_90a into cudalibrarysamples_b200/libb200spmv.so (+ libb200gen.so, libb200spsv.so).
 
     extra_flags / out_path / tag build a tuning variant of the product library (scripts/sweep.py) next to the default."""
     variant = bool(extra_flags) or out_path is not None
@@ -93,6 +97,8 @@ def build_native(force: bool = False, verbose: bool = False, extra_flags=(), out
         _compile_and_link(SOURCES, LIB_PATH, build_dir, [], log)
     if force or _stale(GEN_LIB_PATH, GEN_SOURCES):
         _compile_and_link(GEN_SOURCES, GEN_LIB_PATH, os.path.join(build_dir, "gen"), [], log)
+    if force or _stale(SPSV_LIB_PATH, SPSV_SOURCES):
+        _compile_and_link(SPSV_SOURCES, SPSV_LIB_PATH, os.path.join(build_dir, "spsv"), [], log)
     if log:
         with open(os.path.join(build_dir, "build.log"), "w") as f:
             f.write("\n".join(log))

@@ -29,6 +29,7 @@ REAL_CUSPARSE_CANDIDATES = (
 )
 
 _shim = None
+_spsv = None
 _gen = None
 _real = None
 _real_path = None
@@ -83,6 +84,24 @@ def shim(build_if_missing: bool = False) -> C.CDLL:
         lib.b200spmv_version.restype = C.c_char_p
         _shim = lib
     return _shim
+
+
+def spsv() -> C.CDLL:
+    """libb200spsv.so, the opt-in CSR triangular solve (include/b200spsv.h). Raises if it has not been built."""
+    global _spsv
+    if _spsv is None:
+        # like shim(): the library must dlopen the very libcusparse instance that creates the handles we pass to it
+        os.environ["B200SPMV_CUSPARSE"] = real_cusparse_path()
+        path = _build.SPSV_LIB_PATH
+        if not os.path.exists(path):
+            raise RuntimeError(f"{path} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_90a). "
+                               "There is no CPU fallback.")
+        lib = C.CDLL(path, mode=C.RTLD_LOCAL)
+        lib.b200spsv_csr_workspace_bytes.restype = C.c_size_t
+        lib.b200spsv_csr_workspace_bytes.argtypes = [C.c_int64, C.c_int64, C.c_int]
+        lib.b200spsv_version.restype = C.c_char_p
+        _spsv = lib
+    return _spsv
 
 
 def gen() -> C.CDLL:
