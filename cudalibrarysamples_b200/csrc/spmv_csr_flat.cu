@@ -28,6 +28,7 @@
 #include "spmv_common.cuh"
 #include "config.h"
 #include "../../include/b200spmv.h"
+#include <vector>
 
 namespace b200 {
 
@@ -69,6 +70,18 @@ constexpr int FLAT_BATCH32 = (2 * B200_FLAT_BATCH <= B200_FLAT_STEPS) ? 2 * B200
 constexpr int SCAN_ITEMS = 2048;                   // items per block of the preprocessing scans
 static_assert(FLAT_STEPS % FLAT_BATCH64 == 0 && FLAT_STEPS % FLAT_BATCH32 == 0, "steps per chunk must be a multiple of the batch");
 
+// Hot columns of x.  Preprocess picks the most-used columns whose values fit B200_FLAT_HOT_BYTES, and every SpMV first packs
+// their x values densely (xh) so the gather of csr_flat_kernel finds them on fewer, fully used cache lines.  On R-MAT the
+// hot columns are scattered over lines shared with cold columns; packed, more of the gathers hit L1.
+#ifndef B200_FLAT_HOT_BYTES
+#define B200_FLAT_HOT_BYTES (64 * 1024)   // swept over 0 / 64 / 96 / 128 / 160 KB on the H100: scripts/sweep.py flat_hot
+#endif
+constexpr int HOT_BYTES = B200_FLAT_HOT_BYTES;
+constexpr int HOT_MAX = HOT_BYTES / 4;              // slots of the hot list: fp32 fits twice as many values as fp64
+constexpr int HOT_MIN_PERMILLE = 200;               // the hot columns must take at least this share of nnz, else no hot plan
+constexpr int HOT_BINS = 1 << 16;                   // column-count histogram: bin n = columns used n times, the last bin >= n
+static_assert(HOT_BYTES % 8 == 0, "B200_FLAT_HOT_BYTES must be a multiple of 8");
+
 struct FlatPlan {
     unsigned* endmask;    // [nctas * 64]   zero-padded behind nnz
     int*      chunk_run;  // [nctas * 8 + 1]
@@ -76,8 +89,13 @@ struct FlatPlan {
     double*   cta_first;  // [nctas]  sum in front of the CTA's first row end (whole CTA if no row ends in it)
     double*   cta_last;   // [nctas]  sum behind the CTA's last row end
     int*      cta_flags;  // [nctas]  1: at least one row ends in this CTA
-    int*      ctl;        // [0] nruns (non-empty rows), [1] steps without a row end, [2] steps
+    int*      ctl;        // [0] nruns (non-empty rows), [1] steps without a row end, [2] steps, [4] hot columns H, [5] threshold,
+                          // [6..7] non-zeros in columns of the last histogram bin (uint64)
     int*      scratch;    // block sums of the scans
+    int*      colp;       // [nchunks * 256]  ~j for hot slot j, else the 0-based column; 0 behind nnz.  Column counts before that.
+    int*      hot;        // [HOT_MAX]        0-based columns of the hot slots, ascending
+    void*     xh;         // [HOT_BYTES]      x[hot[j]], refreshed by every SpMV with H > 0
+    unsigned* bins;       // [HOT_BINS]
 };
 
 static inline size_t flat_align(size_t v) { return (v + 255) / 256 * 256; }
@@ -87,7 +105,9 @@ static inline int64_t flat_num_chunks_padded(int64_t nnz) { return (nnz + FLAT_P
 static size_t flat_layout(int64_t rows, int64_t nnz, void* ws, FlatPlan* p) {
     const size_t nchunks = (size_t)flat_num_chunks_padded(nnz);
     const size_t nctas = nchunks;                                  // upper bound for every FLAT_WARPS (one CTA per chunk)
-    const size_t nscan = (size_t)((rows > (int64_t)nchunks ? rows : (int64_t)nchunks) / SCAN_ITEMS + 2);
+    const size_t ncolp = HOT_BYTES > 0 ? nchunks * PLAN_CHUNK : 0; // also the largest column count the hot plan takes
+    const int64_t nscan_items = rows > (int64_t)ncolp ? rows : (int64_t)ncolp;
+    const size_t nscan = (size_t)((nscan_items > (int64_t)nchunks ? nscan_items : (int64_t)nchunks) / SCAN_ITEMS + 2);
     size_t o = 0;
     const size_t o_mask = o;  o = flat_align(o + nchunks * PLAN_STEPS * sizeof(unsigned));
     const size_t o_crun = o;  o = flat_align(o + (nchunks + 1) * sizeof(int));
@@ -97,11 +117,17 @@ static size_t flat_layout(int64_t rows, int64_t nnz, void* ws, FlatPlan* p) {
     const size_t o_fl   = o;  o = flat_align(o + nctas * sizeof(int));
     const size_t o_ctl  = o;  o = flat_align(o + 64);
     const size_t o_scr  = o;  o = flat_align(o + nscan * sizeof(int));
+    const bool   hot = ncolp > 0;
+    const size_t o_colp = o;  o = flat_align(o + ncolp * sizeof(int));
+    const size_t o_hot  = o;  o = flat_align(o + (hot ? HOT_MAX * sizeof(int) : 0));
+    const size_t o_xh   = o;  o = flat_align(o + (hot ? HOT_BYTES : 0));
+    const size_t o_bins = o;  o = flat_align(o + (hot ? HOT_BINS * sizeof(unsigned) : 0));
     if (p) {
         char* b = (char*)ws;
         p->endmask = (unsigned*)(b + o_mask); p->chunk_run = (int*)(b + o_crun); p->nzrow = (int*)(b + o_nzr);
         p->cta_first = (double*)(b + o_cf); p->cta_last = (double*)(b + o_cl); p->cta_flags = (int*)(b + o_fl);
         p->ctl = (int*)(b + o_ctl); p->scratch = (int*)(b + o_scr);
+        p->colp = (int*)(b + o_colp); p->hot = (int*)(b + o_hot); p->xh = (void*)(b + o_xh); p->bins = (unsigned*)(b + o_bins);
     }
     return o;
 }
@@ -235,15 +261,79 @@ __global__ void flat_finish_kernel(FlatPlan p, int64_t rows, int64_t nchunks, in
     if ((threadIdx.x & 31) == 0 && quiet) atomicAdd(p.ctl + 1, quiet);
 }
 
+// hot plan: uses per column (colp doubles as the counter array), then how many columns have each use count
+__global__ void flat_hot_count_kernel(const int* __restrict__ col, int base, int64_t nnz, int64_t cols, int* __restrict__ cnt) {
+    for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nnz; k += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t c = (int64_t)__ldg(col + k) - base;
+        if (c >= 0 && c < cols) atomicAdd(cnt + c, 1);
+    }
+}
+
+__global__ void flat_hot_bins_kernel(const int* __restrict__ cnt, int64_t cols, unsigned* __restrict__ bins,
+                                     unsigned long long* __restrict__ last_bin_nnz) {
+    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < cols; c += (int64_t)gridDim.x * blockDim.x) {
+        const int n = cnt[c];
+        if (n < 2) continue;
+        atomicAdd(bins + min(n, HOT_BINS - 1), 1u);
+        if (n >= HOT_BINS - 1) atomicAdd(last_bin_nnz, (unsigned long long)n);
+    }
+}
+
+struct HotFlag {
+    const int* cnt;
+    int        tau;
+    __device__ __forceinline__ int operator()(int64_t c) const { return cnt[c] >= tau ? 1 : 0; }
+};
+struct EmitHot {
+    int* hot;
+    __device__ __forceinline__ void operator()(int64_t c, int rank, int v) const { if (v) hot[rank] = (int)c; }
+};
+
+// colp[k] = ~j if column col[k] - base is hot slot j (binary search of the ascending hot list), else col[k] - base
+__global__ void flat_hot_colp_kernel(const int* __restrict__ col, int base, int64_t nnz, int64_t npad, const int* __restrict__ hot,
+                                     int nhot, int tau, int* __restrict__ colp, int* __restrict__ ctl) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) { ctl[4] = nhot; ctl[5] = tau; }
+    for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < npad; k += (int64_t)gridDim.x * blockDim.x) {
+        int v = 0;                                          // behind nnz: a column that is never hot
+        if (k < nnz) {
+            v = __ldg(col + k) - base;
+            int lo = 0, hi = nhot;
+            while (lo < hi) {
+                const int mid = (lo + hi) >> 1;
+                if (__ldg(hot + mid) < v) lo = mid + 1; else hi = mid;
+            }
+            if (lo < nhot && __ldg(hot + lo) == v) v = ~lo;
+        }
+        colp[k] = v;
+    }
+}
+
+// The threshold: the smallest tau >= 2 whose columns (used >= tau times) fit `slots`; no hot plan (0) when even the last bin does
+// not fit or the hot columns take less than HOT_MIN_PERMILLE of nnz.
+static int flat_hot_choose(const unsigned* bins, unsigned long long last_bin_nnz, int64_t nnz, int64_t slots, int* tau_out) {
+    long long h = 0, covered = (long long)last_bin_nnz;
+    int tau = 0;
+    for (int t = HOT_BINS - 1; t >= 2; t--) {
+        if (h + bins[t] > slots) break;
+        h += bins[t];
+        if (t < HOT_BINS - 1) covered += (long long)t * bins[t];
+        tau = t;
+    }
+    *tau_out = tau;
+    if (tau == 0 || h == 0 || covered * 1000 < (long long)HOT_MIN_PERMILLE * nnz) return 0;
+    return (int)h;
+}
+
 // ------------------------------------------------------------------------------------------------
 // SpMV
 // ------------------------------------------------------------------------------------------------
 template <typename T>
 struct FlatArgs {
     const int* off;
-    const int* col;
+    const int* col;       // the caller's col_ind, or colp of a hot plan (then base == 0)
     const T*   val;
     const T*   x;
+    const T*   xh;        // packed hot values: read for col < 0
     T*         y;
     int        base;
     int        rows;
@@ -319,7 +409,8 @@ __global__ void __launch_bounds__(FLAT_BLOCK, B200_FLAT_MIN_CTAS) csr_flat_kerne
             if (n0 + kb * 32 >= n1) break;                 // warp-uniform: the matrix' last chunk may be short
             T p[FLAT_BATCH];
 #pragma unroll
-            for (int k = 0; k < FLAT_BATCH; k++) p[k] = (n0 + (kb + k) * 32 + lane < n1) ? vv[k] * __ldg(xp + cc[k]) : T(0);
+            for (int k = 0; k < FLAT_BATCH; k++)
+                p[k] = (n0 + (kb + k) * 32 + lane < n1) ? vv[k] * (cc[k] < 0 ? __ldg(a.xh + ~cc[k]) : __ldg(xp + cc[k])) : T(0);
             if (kb + FLAT_BATCH < FLAT_STEPS && n0 + (kb + FLAT_BATCH) * 32 < n1) issue(kb + FLAT_BATCH);
 #pragma unroll
             for (int k = 0; k < FLAT_BATCH; k++) {
@@ -433,20 +524,33 @@ __global__ void flat_scale_y_kernel(T* __restrict__ y, int64_t rows, Scalars<T> 
 }
 
 template <typename T>
+__global__ void flat_hot_pack_kernel(const int* __restrict__ hot, int nhot, const T* __restrict__ x, T* __restrict__ xh) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < nhot) xh[j] = __ldg(x + __ldg(hot + j));
+}
+
+template <typename T>
 static int launch_flat(cudaStream_t stream, int64_t rows, int64_t nnz, const void* off, const void* col, const void* val, int base,
-                       const void* alpha, const void* beta, int on_device, const void* x, void* y, void* ws) {
+                       const void* alpha, const void* beta, int on_device, const void* x, void* y, void* ws, int nhot) {
+    if (nhot < 0 || (int64_t)nhot * (int64_t)sizeof(T) > HOT_BYTES || (nhot > 0 && nnz == 0)) return -1;
     FlatArgs<T> a;
     a.off = (const int*)off; a.col = (const int*)col; a.val = (const T*)val; a.x = (const T*)x; a.y = (T*)y;
     a.base = base; a.rows = (int)rows; a.nnz = (int)nnz;
     if (on_device) { a.s.alpha = T(0); a.s.beta = T(0); a.s.alpha_dev = (const T*)alpha; a.s.beta_dev = (const T*)beta; }
     else { a.s.alpha = *(const T*)alpha; a.s.beta = *(const T*)beta; a.s.alpha_dev = nullptr; a.s.beta_dev = nullptr; }
     flat_layout(rows, nnz, ws, &a.plan);
+    a.xh = (const T*)a.plan.xh;
     stats().last_csr_kernel = sizeof(T) == 8 ? "b200::csr_flat_kernel<double>" : "b200::csr_flat_kernel<float>";
     if (nnz == 0) {
         int64_t blocks = (rows + 255) / 256;
         if (blocks > 132 * 16) blocks = 132 * 16;
         flat_scale_y_kernel<T><<<(unsigned)blocks, 256, 0, stream>>>((T*)y, rows, a.s);
         return (int)cudaGetLastError();
+    }
+    if (nhot > 0) {                                         // same products in the same order: only where x[c] is read from changes
+        flat_hot_pack_kernel<T><<<(unsigned)((nhot + 255) / 256), 256, 0, stream>>>(a.plan.hot, nhot, (const T*)x, (T*)a.plan.xh);
+        a.col = a.plan.colp;
+        a.base = 0;
     }
     const int64_t nctas = flat_num_ctas(nnz);
     csr_flat_kernel<T><<<(unsigned)nctas, FLAT_BLOCK, 0, stream>>>(a);
@@ -523,16 +627,82 @@ void b200spmv_csr_flat_params(int32_t* warp_chunk, int32_t* cta_nnz, int32_t* pl
     if (plan_chunk) *plan_chunk = PLAN_CHUNK;
 }
 
+int b200spmv_csr_flat_hot_analyze(void* stream_, int dtype, int64_t rows, int64_t cols, int64_t nnz, const void* col_ind, int32_t base,
+                                  void* workspace, int32_t* hot_out) {
+    if (!hot_out) return -1;
+    *hot_out = 0;
+    if (rows < 0 || cols < 0 || nnz < 0 || rows > INT32_MAX - 2 || cols > INT32_MAX || nnz > INT32_MAX - 65536 || !workspace ||
+        (nnz > 0 && !col_ind) || (dtype != 0 && dtype != 1))
+        return -1;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    FlatPlan p;
+    flat_layout(rows, nnz, workspace, &p);
+    cudaError_t e = cudaMemsetAsync(p.ctl + 4, 0, 4 * sizeof(int), stream);
+    if (e != cudaSuccess) return (int)e;
+    const int64_t npad = flat_num_chunks_padded(nnz) * PLAN_CHUNK;
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    if (cudaStreamIsCapturing(stream, &cap) != cudaSuccess) cap = cudaStreamCaptureStatusNone;
+    // the counters live in colp: no hot plan for more columns than that holds, nor under capture (the threshold is read back)
+    if (HOT_BYTES == 0 || nnz == 0 || cols > npad || cap != cudaStreamCaptureStatusNone) return 0;
+    const int* col = (const int*)col_ind;
+    unsigned long long* last_bin_nnz = (unsigned long long*)(p.ctl + 6);
+    if ((e = cudaMemsetAsync(p.colp, 0, (size_t)cols * sizeof(int), stream)) != cudaSuccess) return (int)e;
+    if ((e = cudaMemsetAsync(p.bins, 0, HOT_BINS * sizeof(unsigned), stream)) != cudaSuccess) return (int)e;
+    int64_t blocks = (nnz + 255) / 256;
+    if (blocks > 132 * 32) blocks = 132 * 32;
+    flat_hot_count_kernel<<<(unsigned)blocks, 256, 0, stream>>>(col, base, nnz, cols, p.colp);
+    int64_t cblocks = (cols + 255) / 256;
+    if (cblocks > 132 * 32) cblocks = 132 * 32;
+    if (cblocks < 1) cblocks = 1;
+    flat_hot_bins_kernel<<<(unsigned)cblocks, 256, 0, stream>>>(p.colp, cols, p.bins, last_bin_nnz);
+    if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
+    std::vector<unsigned> bins(HOT_BINS);
+    unsigned long long last = 0;
+    if ((e = cudaMemcpyAsync(bins.data(), p.bins, HOT_BINS * sizeof(unsigned), cudaMemcpyDeviceToHost, stream)) != cudaSuccess ||
+        (e = cudaMemcpyAsync(&last, last_bin_nnz, sizeof last, cudaMemcpyDeviceToHost, stream)) != cudaSuccess ||
+        (e = cudaStreamSynchronize(stream)) != cudaSuccess)
+        return (int)e;
+    int tau = 0;
+    const int nhot = flat_hot_choose(bins.data(), last, nnz, HOT_BYTES / (dtype == 1 ? 8 : 4), &tau);
+    if (nhot == 0) return 0;
+    const int64_t nb = (cols + SCAN_ITEMS - 1) / SCAN_ITEMS;      // the hot list, ascending: a scan over the columns
+    HotFlag v{p.colp, tau};
+    scan_block_sums_kernel<<<(unsigned)nb, 256, 0, stream>>>(v, cols, p.scratch);
+    scan_of_block_sums_kernel<<<1, 1024, 0, stream>>>(p.scratch, nb, p.ctl + 8);
+    scan_emit_kernel<<<(unsigned)nb, 256, 0, stream>>>(v, EmitHot{p.hot}, cols, p.scratch);
+    int64_t kb = (npad + 255) / 256;
+    if (kb > 132 * 32) kb = 132 * 32;
+    flat_hot_colp_kernel<<<(unsigned)kb, 256, 0, stream>>>(col, base, nnz, npad, p.hot, nhot, tau, p.colp, p.ctl);
+    if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
+    *hot_out = nhot;
+    return 0;
+}
+
+void b200spmv_csr_flat_hot_offsets(int64_t rows, int64_t nnz, size_t* colp, size_t* hot) {
+    FlatPlan p;
+    flat_layout(rows, nnz, nullptr, &p);
+    if (colp) *colp = (size_t)((char*)p.colp - (char*)nullptr);
+    if (hot) *hot = (size_t)((char*)p.hot - (char*)nullptr);
+}
+
+void b200spmv_csr_flat_hot_params(int32_t* hot_bytes, int32_t* min_share_permille, int32_t* bins) {
+    if (hot_bytes) *hot_bytes = HOT_BYTES;
+    if (min_share_permille) *min_share_permille = HOT_MIN_PERMILLE;
+    if (bins) *bins = HOT_BINS;
+}
+
 int b200spmv_csr_flat_mv(void* stream, int dtype, int64_t rows, int64_t cols, int64_t nnz, const void* row_offsets,
                          const void* col_ind, const void* values, int32_t base, const void* alpha, const void* beta,
-                         int scalars_on_device, const void* x, void* y, void* workspace) {
+                         int scalars_on_device, const void* x, void* y, void* workspace, int32_t hot) {
     if (rows < 0 || cols < 0 || nnz < 0 || !alpha || !beta) return -1;
     if (rows == 0) return 0;
     if (!y || !workspace || !row_offsets || (nnz > 0 && (!col_ind || !values || !x))) return -1;
     if (dtype == 0)
-        return launch_flat<float>((cudaStream_t)stream, rows, nnz, row_offsets, col_ind, values, base, alpha, beta, scalars_on_device, x, y, workspace);
+        return launch_flat<float>((cudaStream_t)stream, rows, nnz, row_offsets, col_ind, values, base, alpha, beta, scalars_on_device, x, y,
+                                  workspace, hot);
     if (dtype == 1)
-        return launch_flat<double>((cudaStream_t)stream, rows, nnz, row_offsets, col_ind, values, base, alpha, beta, scalars_on_device, x, y, workspace);
+        return launch_flat<double>((cudaStream_t)stream, rows, nnz, row_offsets, col_ind, values, base, alpha, beta, scalars_on_device, x, y,
+                                   workspace, hot);
     return -1;
 }
 

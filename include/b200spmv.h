@@ -59,16 +59,31 @@ B200SPMV_EXPORT size_t  b200spmv_csr_plan_ctl_offset(int64_t rows, int64_t nnz);
 B200SPMV_EXPORT size_t  b200spmv_csr_plan_split_offset(int64_t rows, int64_t nnz);
 
 /* CSR, "flat" plan (spmv_csr_flat.cu): a second, larger structure-only plan -- one bit per non-zero marking row ends, a
- * run counter per 256 non-zeros, the list of non-empty rows -- built once by cusparseSpMV_preprocess for matrices with
+ * run counter per 256 non-zeros, the list of non-empty rows, and the hot-column copy of col_ind below -- built once by cusparseSpMV_preprocess for matrices with
  * long / skewed rows; the SpMV kernel then needs no row offsets, no shared-memory staging and no barriers inside a warp's
  * chunk.  Same call sites as above (spmv_csr_example.c:104-112: preprocess, then SpMV). */
 B200SPMV_EXPORT size_t b200spmv_csr_flat_workspace_bytes(int64_t rows, int64_t nnz);
 B200SPMV_EXPORT int    b200spmv_csr_flat_analyze(void* stream, int64_t rows, int64_t nnz, const void* row_offsets,
                                                  int32_t base, void* workspace);
+/* The hot-column part of the flat plan, built after _flat_analyze in the same workspace (needs cols <= nnz rounded up to
+ * 2048, else no hot plan).  The hot columns are those used at least tau times, tau >= 2 the smallest threshold whose columns
+ * fit b200spmv_csr_flat_hot_params' byte budget for this dtype; they get slots 0..H-1 in ascending column order.  colp
+ * (int32 per non-zero, 0 behind nnz up to the padded chunk count) holds ~slot for a hot column, else the 0-based column.
+ * H = 0 when the hot columns take less than min_share_permille / 1000 of nnz, or while the stream is being captured.
+ * Reads a column-count histogram back: synchronises the stream once.  *hot_out = H, to be passed to _flat_mv; the
+ * workspace's control words (see _flat_plan_offsets) hold H at [4] and tau at [5].  The plan depends on col_ind only, so
+ * it stays valid when the values change. */
+B200SPMV_EXPORT int    b200spmv_csr_flat_hot_analyze(void* stream, int dtype, int64_t rows, int64_t cols, int64_t nnz,
+                                                     const void* col_ind, int32_t base, void* workspace, int32_t* hot_out);
+B200SPMV_EXPORT void   b200spmv_csr_flat_hot_offsets(int64_t rows, int64_t nnz, size_t* colp, size_t* hot);
+B200SPMV_EXPORT void   b200spmv_csr_flat_hot_params(int32_t* hot_bytes, int32_t* min_share_permille, int32_t* bins);
+/* hot: the H of b200spmv_csr_flat_hot_analyze, or 0 (the kernel then reads col_ind).  With H > 0 a small kernel first
+ * packs x[hot[j]] into the workspace and csr_flat_kernel reads colp: the same products in the same order, so y is
+ * bit-identical to the H = 0 call. */
 B200SPMV_EXPORT int    b200spmv_csr_flat_mv(void* stream, int dtype, int64_t rows, int64_t cols, int64_t nnz,
                                             const void* row_offsets, const void* col_ind, const void* values,
                                             int32_t base, const void* alpha, const void* beta, int scalars_on_device,
-                                            const void* x, void* y, void* workspace);
+                                            const void* x, void* y, void* workspace, int32_t hot);
 /* byte offsets of the flat plan's arrays inside its workspace: endmask (uint32 per 32 non-zeros, zero-padded to a
  * multiple of 64 words), chunk_run (int32 per 256 non-zeros, padded to whole groups of 8, + 1), nzrow (int32, rows + 2), control words
  * {non-empty rows, steps without a row end, steps} -- read back by the bit-exact preprocessing tests */

@@ -107,6 +107,9 @@ if os.environ.get("SWEEP_SET") == "flat4":
     # csr_flat_kernel: deeper load batches / more resident CTAs (the fp32 kernel has registers to spare)
     VARIANTS = {f"flat4_occ{o}_k{k}_w{w}_s{st}": dict(FLAT=(o, k, w, st)) for (o, k, w, st) in
                 [(10, 8, 4, 8), (12, 8, 4, 8), (12, 4, 4, 8), (8, 8, 4, 8)]}
+if os.environ.get("SWEEP_SET") == "flat_hot":
+    # csr_flat_kernel: byte budget of the packed hot columns of x (0 = no hot plan)
+    VARIANTS = {f"flat_hot{kb}k": dict(FLATHOT=kb) for kb in (0, 64, 96, 128, 160)}
 if os.environ.get("SWEEP_SET") == "short":
     # csr_short_kernel: (warps per CTA, load steps per pass, resident CTAs)
     VARIANTS = {f"short_w{w}_s{st}_occ{o}": dict(SHORT=(w, st, o)) for (w, st, o) in
@@ -121,6 +124,8 @@ def flags(v):
         return [f"-DB200_FLAT_MIN_CTAS={o}", f"-DB200_FLAT_BATCH={k}", f"-DB200_FLAT_WARPS={w}", f"-DB200_FLAT_STEPS={st}"]
     if "FLAT3" in v:
         return [f"-DB200_FLAT_QUIET_BALLOT={v['FLAT3'][0]}", f"-DB200_FLAT_EMPTY_TAIL={v['FLAT3'][1]}"]
+    if "FLATHOT" in v:
+        return [f"-DB200_FLAT_HOT_BYTES={v['FLATHOT'] * 1024}"]
     if "SHORT" in v:
         w, st, o = v["SHORT"]
         return [f"-DB200_SHORT_WARPS={w}", f"-DB200_SHORT_STEPS={st}", f"-DB200_SHORT_MIN_CTAS={o}"]
@@ -153,7 +158,7 @@ def build():
         out = os.path.join(VDIR, f"libb200spmv_{tag}.so")
         b.build_native(extra_flags=flags(v), out_path=out, tag="v_" + tag)
         log = open(os.path.join(ROOT, "cudalibrarysamples_b200", "build", "v_" + tag, "build.log")).read()
-        i = log.find("csr_short_kernelIdEE") if "SHORT" in v else log.find("csr_flat_kernelIdEE") if ("FLAT" in v or "FLAT3" in v) else log.find("csr_seg_kernelIdEE") if "SEG" in v else log.find("csr_rowwise_kernelIdEE") if "RW" in v else log.find("csr_ws_kernelIdEE") if "WS" in v else max(log.find("csr_pipe_kernelIdEE"), log.find("csr_tile_kernelIdEE")) if "-DB200_CSR_KERNEL=0" not in " ".join(flags(v)) else log.find("csr_tile_kernelIdEE")
+        i = log.find("csr_short_kernelIdEE") if "SHORT" in v else log.find("csr_flat_kernelIdEE") if ("FLAT" in v or "FLAT3" in v or "FLATHOT" in v) else log.find("csr_seg_kernelIdEE") if "SEG" in v else log.find("csr_rowwise_kernelIdEE") if "RW" in v else log.find("csr_ws_kernelIdEE") if "WS" in v else max(log.find("csr_pipe_kernelIdEE"), log.find("csr_tile_kernelIdEE")) if "-DB200_CSR_KERNEL=0" not in " ".join(flags(v)) else log.find("csr_tile_kernelIdEE")
         regs = log[i:i + 400].split("Used ")[1].split(",")[0] if i >= 0 else "?"
         print(tag, regs)
 
