@@ -138,6 +138,14 @@ __global__ void __launch_bounds__(256) spmm_transpose_b_kernel(const T* __restri
     }
 }
 
+// The same transpose as a host call on `stream` (dtype 0 = fp32, 1 = fp64): sddmm_csr.cu uses it to make an operand K-contiguous.
+int transpose_col_to_row_major(cudaStream_t stream, int dtype, const void* B, int64_t ldb, void* Bt, int64_t cols, int64_t n) {
+    const dim3 tg((unsigned)((cols + 31) / 32), (unsigned)((n + 31) / 32));
+    if (dtype == 1) spmm_transpose_b_kernel<double><<<tg, 256, 0, stream>>>((const double*)B, (long long)ldb, (double*)Bt, (int)cols, (int)n);
+    else spmm_transpose_b_kernel<float><<<tg, 256, 0, stream>>>((const float*)B, (long long)ldb, (float*)Bt, (int)cols, (int)n);
+    return (int)cudaGetLastError();
+}
+
 constexpr int SPMM_MIN_N_FOR_TRANSPOSE = 4;      // below that a strided walk over column-major B costs less than the extra pass
 
 template <typename T>

@@ -82,6 +82,7 @@ def shim(build_if_missing: bool = False) -> C.CDLL:
         lib.b200spmv_csr_plan_split_offset.restype = C.c_size_t
         lib.b200spmv_csr_num_tiles.restype = C.c_int64
         lib.b200spmv_version.restype = C.c_char_p
+        lib.b200sddmm_csr_workspace_bytes.restype = C.c_size_t
         _shim = lib
     return _shim
 

@@ -137,6 +137,28 @@ B200SPMV_EXPORT int b200spmm_csr(void* stream, int dtype, int64_t rows, int64_t 
                                  const void* alpha, const void* beta, int scalars_on_device, const void* B, int64_t ldb,
                                  int b_row_major, void* C, int64_t ldc, int c_row_major);
 
+/* Sampled dense-dense product (sddmm_csr.cu): C = alpha * (op(A) * op(B)) o spy(C) + beta * C for a CSR C of m x n (int32
+ * offsets / columns, `values` updated in place, once per entry, no atomics), op(A) m x k and op(B) k x n dense.  Replaces
+ * cusparseSDDMM (cuSPARSE/sddmm_csr/sddmm_csr_example.c:114-134).  Any dense layout is passed as element strides:
+ *   op(A)(i, k) = A[i * sai + k * sak],   op(B)(k, j) = B[k * sbk + j * sbj]   (strides >= 0).
+ * batch >= 1 products run in one launch; matrix b of the batch uses offsets + b * off_stride, col_ind / values + b * colval_stride,
+ * A + b * a_stride, B + b * b_stride (elements; 0 = shared by the batch; colval_stride >= nnz when batch > 1).
+ * workspace: b200sddmm_csr_workspace_bytes() bytes, 16-byte aligned, where an operand that is not K-contiguous (its k stride is not
+ * 1) is copied to a tight K-contiguous matrix on every call; a NULL, misaligned or smaller buffer makes the kernel read that operand
+ * with strided loads instead.  beta == 0 never reads C's values.  K = 0 gives C = beta * C. */
+B200SPMV_EXPORT size_t b200sddmm_csr_workspace_bytes(int dtype, int64_t m, int64_t n, int64_t k, int64_t sai, int64_t sak, int64_t sbk,
+                                                     int64_t sbj, int batch, int64_t a_stride, int64_t b_stride);
+B200SPMV_EXPORT int b200sddmm_csr(void* stream, int dtype, int64_t m, int64_t n, int64_t k, int64_t nnz, const void* row_offsets,
+                                  const void* col_ind, void* values, int32_t base, const void* alpha, const void* beta,
+                                  int scalars_on_device, const void* A, int64_t sai, int64_t sak, const void* B, int64_t sbk,
+                                  int64_t sbj, int batch, int64_t off_stride, int64_t colval_stride, int64_t a_stride,
+                                  int64_t b_stride, void* workspace, size_t workspace_bytes);
+/* sddmm_csr_kernel's constants: consecutive non-zeros per warp, entries a lane group has in flight, the width of the vector loads of
+ * the K-contiguous path, the widest lane group.  G lanes share one entry: G = the smallest power of two with G * V >= k, at most
+ * max_group, where V = vec_bytes / sizeof(value) on the K-contiguous path (k a multiple of V, operands 16-byte aligned) and 1 on
+ * the strided path; a warp steps through its chunk 32 / G * entries_per_group entries at a time. */
+B200SPMV_EXPORT void b200sddmm_params(int32_t* warp_chunk, int32_t* entries_per_group, int32_t* vec_bytes, int32_t* max_group);
+
 /* The BLAS-1 part of a CG iteration, fused, all scalars in DEVICE memory (no host synchronisation, CUDA-graph capturable).
  * Replaces the cublasDdot / cublasDaxpy / cublasDnrm2 / cublasDscal calls between two cusparseSpMV calls of gpu_CG
  * (cuSPARSE/cg/cg_example.c:226-286).  fp64; vectors 16-byte aligned; `workspace` = b200cg_workspace_bytes() bytes, zeroed
@@ -232,6 +254,12 @@ B200SPMV_EXPORT int b200spmv_route(int format, int op, int alg, int off_type, in
 /* How many products cusparseSpMM would run on our kernel for these descriptors (cusparseSpMatDescr_t / cusparseDnMatDescr_t passed
  * as void*): 0 = the call goes to the closed library, 1 = an ordinary product, N = a strided batch.  Host logic only. */
 B200SPMV_EXPORT int b200spmm_batch_count(const void* matA, const void* matB, const void* matC);
+/* Where cusparseSDDMM_bufferSize / _preprocess / cusparseSDDMM send a call with these descriptors (cusparseDnMatDescr_t A, B and
+ * cusparseSpMatDescr_t C passed as void*, enum values as int): 0 = the closed library (64-bit indices, 16-bit / complex / mixed
+ * types, a compute type other than the value type, non-CSR C, CONJUGATE_TRANSPOSE, an unsupported batch layout,
+ * B200SPMV_FORWARD=1, and where the closed library measured faster: fp64, and fp32 with K > 32 when op(B) is K-contiguous),
+ * 1 = one product on sddmm_csr_kernel, N = a strided batch of N.  Host logic only. */
+B200SPMV_EXPORT int b200sddmm_route(const void* matA, const void* matB, const void* matC, int opA, int opB, int computeType);
 /* name of the main kernel the most recent CSR SpMV launched, e.g. "b200::csr_seg_kernel<double>" (bench.py's roofline.kernel) */
 B200SPMV_EXPORT const char* b200spmv_last_csr_kernel(void);
 
@@ -312,6 +340,16 @@ B200SPMV_EXPORT cusparseStatus_t cusparseSpMM_preprocess(cusparseHandle_t, cuspa
 B200SPMV_EXPORT cusparseStatus_t cusparseSpMM(cusparseHandle_t, cusparseOperation_t, cusparseOperation_t, const void*,
                                               cusparseConstSpMatDescr_t, cusparseConstDnMatDescr_t, const void*,
                                               cusparseDnMatDescr_t, cudaDataType, cusparseSpMMAlg_t, void*);
+/* cusparse.h:6052-6088 -- sddmm_csr_example.c:114-134, sddmm_csr_batched_example.c:146-166 */
+B200SPMV_EXPORT cusparseStatus_t cusparseSDDMM_bufferSize(cusparseHandle_t, cusparseOperation_t, cusparseOperation_t, const void*,
+                                                          cusparseConstDnMatDescr_t, cusparseConstDnMatDescr_t, const void*,
+                                                          cusparseSpMatDescr_t, cudaDataType, cusparseSDDMMAlg_t, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseSDDMM_preprocess(cusparseHandle_t, cusparseOperation_t, cusparseOperation_t, const void*,
+                                                          cusparseConstDnMatDescr_t, cusparseConstDnMatDescr_t, const void*,
+                                                          cusparseSpMatDescr_t, cudaDataType, cusparseSDDMMAlg_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseSDDMM(cusparseHandle_t, cusparseOperation_t, cusparseOperation_t, const void*,
+                                               cusparseConstDnMatDescr_t, cusparseConstDnMatDescr_t, const void*,
+                                               cusparseSpMatDescr_t, cudaDataType, cusparseSDDMMAlg_t, void*);
 #ifdef __cplusplus
 }
 #endif
