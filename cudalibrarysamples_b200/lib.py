@@ -83,6 +83,10 @@ def shim(build_if_missing: bool = False) -> C.CDLL:
         lib.b200spmv_csr_num_tiles.restype = C.c_int64
         lib.b200spmv_version.restype = C.c_char_p
         lib.b200sddmm_csr_workspace_bytes.restype = C.c_size_t
+        i64, vp = C.c_int64, C.c_void_p
+        lib.b200spmm_bell.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, i64, i64, vp, vp, C.c_int32, vp, vp, C.c_int, vp, i64, C.c_int,
+                                      vp, i64, C.c_int]
+        lib.b200spmm_bell_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
         _shim = lib
     return _shim
 

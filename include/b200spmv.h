@@ -137,6 +137,25 @@ B200SPMV_EXPORT int b200spmm_csr(void* stream, int dtype, int64_t rows, int64_t 
                                  const void* alpha, const void* beta, int scalars_on_device, const void* B, int64_t ldb,
                                  int b_row_major, void* C, int64_t ldc, int c_row_major);
 
+/* Blocked-ELL x dense (spmm_bell.cu): C = alpha * A * B + beta * C, A rows x cols in bs x bs blocks, B cols x n, C rows x n.
+ * Replaces cusparseSpMM for Blocked-ELL descriptors (cuSPARSE/spmm_blockedell/spmm_blockedell_example.cpp).
+ *   a_type    : 2 = fp16 (CUDA_R_16F) or 14 = bf16 (CUDA_R_16BF), the type of A's values and of B.
+ *   c_type    : a_type or 0 = fp32 (CUDA_R_32F).  Products are accumulated in fp32; alpha / beta are fp32.
+ *   col_ind   : (rows / bs) x (ell_cols / bs) int32 block columns, row-major, index base `base`; -1 marks an empty slot.
+ *   values    : rows x ell_cols, row-major: row r holds its block-row's blocks side by side, bs values per block.  The values of an
+ *               empty slot are never read, and neither are the rows of B that no block references.
+ *   B, C      : row- or column-major with leading dimensions ldb / ldc (elements, at least the tight one).
+ * rows, cols and ell_cols must be multiples of bs.  bs % 16 == 0 with 16-byte aligned values / B and ldb % 8 == 0 runs on tensor
+ * cores (mma.sync, fp32 accumulators); everything else on a scalar kernel.  Each C entry is written once in a fixed order (no
+ * atomics: identical bits on every call); beta == 0 never reads C.  No workspace, no allocation, no host synchronisation. */
+B200SPMV_EXPORT int b200spmm_bell(void* stream, int a_type, int c_type, int64_t rows, int64_t cols, int64_t n, int64_t bs, int64_t ell_cols,
+                                  const void* col_ind, const void* values, int32_t base, const void* alpha, const void* beta,
+                                  int scalars_on_device, const void* B, int64_t ldb, int b_row_major, void* C, int64_t ldc,
+                                  int c_row_major);
+/* bell_mma_kernel's constants: columns of C per CTA, K slabs of 16 in flight, and the most rows of C a CTA owns (a CTA owns
+ * 64, 32 or 16 rows of one block-row, the largest of these that divides bs). */
+B200SPMV_EXPORT void b200spmm_bell_params(int32_t* n_tile, int32_t* stages, int32_t* max_rows_per_cta);
+
 /* Sampled dense-dense product (sddmm_csr.cu): C = alpha * (op(A) * op(B)) o spy(C) + beta * C for a CSR C of m x n (int32
  * offsets / columns, `values` updated in place, once per entry, no atomics), op(A) m x k and op(B) k x n dense.  Replaces
  * cusparseSDDMM (cuSPARSE/sddmm_csr/sddmm_csr_example.c:114-134).  Any dense layout is passed as element strides:
@@ -260,6 +279,12 @@ B200SPMV_EXPORT int b200spmm_batch_count(const void* matA, const void* matB, con
  * B200SPMV_FORWARD=1, and where the closed library measured faster: fp64, and fp32 with K > 32 when op(B) is K-contiguous),
  * 1 = one product on sddmm_csr_kernel, N = a strided batch of N.  Host logic only. */
 B200SPMV_EXPORT int b200sddmm_route(const void* matA, const void* matB, const void* matC, int opA, int opB, int computeType);
+/* Where cusparseSpMM sends a call with a Blocked-ELL matA (descriptors passed as void*, enum values as int): 1 = b200spmm_bell,
+ * 0 = the closed library.  Native needs NON_TRANSPOSE for both operands, alg DEFAULT or BLOCKED_ELL_ALG1, int32 block columns,
+ * fp16 / bf16 A and B of one type, C of that type or fp32, compute type fp32, no strided batch, rows and cols multiples of the
+ * block size, no B200SPMV_FORWARD=1, and a class measured at least at parity with the closed library (DESIGN.md 3.14).  A shape
+ * mismatch between A, B and C stays native: the call rejects it.  Host logic only. */
+B200SPMV_EXPORT int b200spmm_bell_route(const void* matA, const void* matB, const void* matC, int opA, int opB, int computeType, int alg);
 /* name of the main kernel the most recent CSR SpMV launched, e.g. "b200::csr_seg_kernel<double>" (bench.py's roofline.kernel) */
 B200SPMV_EXPORT const char* b200spmv_last_csr_kernel(void);
 
