@@ -87,6 +87,11 @@ def shim(build_if_missing: bool = False) -> C.CDLL:
         lib.b200spmm_bell.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, i64, i64, vp, vp, C.c_int32, vp, vp, C.c_int, vp, i64, C.c_int,
                                       vp, i64, C.c_int]
         lib.b200spmm_bell_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
+        lib.b200spmm_coo.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, i64, C.c_int,
+                                     vp, i64, C.c_int, C.c_int, i64, i64, i64, vp, C.c_size_t]
+        lib.b200spmm_coo_workspace_bytes.argtypes = [C.c_int, C.c_int, i64, i64, i64, i64, C.c_int, C.c_int, i64]
+        lib.b200spmm_coo_workspace_bytes.restype = C.c_size_t
+        lib.b200spmm_coo_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
         _shim = lib
     return _shim
 

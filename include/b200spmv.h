@@ -137,6 +137,28 @@ B200SPMV_EXPORT int b200spmm_csr(void* stream, int dtype, int64_t rows, int64_t 
                                  const void* alpha, const void* beta, int scalars_on_device, const void* B, int64_t ldb,
                                  int b_row_major, void* C, int64_t ldc, int c_row_major);
 
+/* COO x dense (spmm_coo.cu): C = alpha * op(A) * B + beta * C, A rows x cols in COO (int32 row_ind / col_ind, index base `base`),
+ * op(A) = A (transpose_a = 0) or A^T (1), B op(A).cols x n and C op(A).rows x n, each row- or column-major with leading dimension
+ * ld* (elements).  Replaces cusparseSpMM for COO descriptors (cuSPARSE/spmm_coo/spmm_coo_example.c:110-122).
+ *   batch     : 1..65535 products in one launch; product i uses row_ind / col_ind / values + i * a_stride, B + i * b_stride and
+ *               C + i * c_stride (elements; 0 = shared by the batch; with batch > 1 the outputs must not overlap).
+ *   workspace : b200spmm_coo_workspace_bytes() bytes, 16-byte aligned: per-batch "unsorted" flags (int32 at
+ *               flag_offset + 4 * i of b200spmm_coo_params), the carry slots of the sorted path, and a row-major copy of a
+ *               column-major B (n >= 4).
+ * Row-sorted A with NON_TRANSPOSE runs deterministically without atomics (identical bits on every call); an unsorted A (any
+ * descending pair of row indices, detected on the device), transpose_a = 1, or a NULL / misaligned / too small workspace runs on
+ * the atomic path (B read in place when there is no workspace).  beta == 0 never reads C.  No allocation, no host synchronisation. */
+B200SPMV_EXPORT size_t b200spmm_coo_workspace_bytes(int dtype, int transpose_a, int64_t rows, int64_t cols, int64_t n, int64_t nnz,
+                                                    int b_row_major, int batch, int64_t b_stride);
+B200SPMV_EXPORT int b200spmm_coo(void* stream, int dtype, int transpose_a, int64_t rows, int64_t cols, int64_t n, int64_t nnz,
+                                 const void* row_ind, const void* col_ind, const void* values, int32_t base, const void* alpha,
+                                 const void* beta, int scalars_on_device, const void* B, int64_t ldb, int b_row_major, void* C,
+                                 int64_t ldc, int c_row_major, int batch, int64_t a_stride, int64_t b_stride, int64_t c_stride,
+                                 void* workspace, size_t workspace_bytes);
+/* the COO SpMM kernels' constants: consecutive non-zeros per warp chunk, columns of B / C per warp, and the byte offset of the
+ * per-batch unsorted flags in the workspace (1 after a call = the atomic path ran for that batch) */
+B200SPMV_EXPORT void b200spmm_coo_params(int32_t* chunk_nnz, int32_t* panel_cols, int64_t* flag_offset);
+
 /* Blocked-ELL x dense (spmm_bell.cu): C = alpha * A * B + beta * C, A rows x cols in bs x bs blocks, B cols x n, C rows x n.
  * Replaces cusparseSpMM for Blocked-ELL descriptors (cuSPARSE/spmm_blockedell/spmm_blockedell_example.cpp).
  *   a_type    : 2 = fp16 (CUDA_R_16F) or 14 = bf16 (CUDA_R_16BF), the type of A's values and of B.
@@ -285,6 +307,13 @@ B200SPMV_EXPORT int b200sddmm_route(const void* matA, const void* matB, const vo
  * block size, no B200SPMV_FORWARD=1, and a class measured at least at parity with the closed library (DESIGN.md 3.14).  A shape
  * mismatch between A, B and C stays native: the call rejects it.  Host logic only. */
 B200SPMV_EXPORT int b200spmm_bell_route(const void* matA, const void* matB, const void* matC, int opA, int opB, int computeType, int alg);
+/* Where cusparseSpMM_bufferSize / _preprocess / cusparseSpMM send a call with a COO matA (descriptors passed as void*, enum values as
+ * int): 0 = the closed library, N >= 1 = N products on b200spmm_coo (a strided batch when N > 1).  Native needs opA NON_TRANSPOSE or
+ * TRANSPOSE, opB NON_TRANSPOSE, alg DEFAULT / COO_ALG1 / COO_ALG3 / COO_ALG4 (COO_ALG2 promises bit-wise reproducibility for any entry
+ * order and is forwarded), int32 indices, fp32 / fp64 A, B, C and compute of one type, a batch layout b200spmm_coo serves, no
+ * B200SPMV_FORWARD=1, and a class measured at least at parity with the closed library (DESIGN.md 3.15).  A shape mismatch stays
+ * native: the call rejects it.  Host logic only. */
+B200SPMV_EXPORT int b200spmm_coo_route(const void* matA, const void* matB, const void* matC, int opA, int opB, int computeType, int alg);
 /* name of the main kernel the most recent CSR SpMV launched, e.g. "b200::csr_seg_kernel<double>" (bench.py's roofline.kernel) */
 B200SPMV_EXPORT const char* b200spmv_last_csr_kernel(void);
 
@@ -335,6 +364,8 @@ B200SPMV_EXPORT cusparseStatus_t cusparseCooSetPointers(cusparseSpMatDescr_t, vo
 B200SPMV_EXPORT cusparseStatus_t cusparseSpMatSetValues(cusparseSpMatDescr_t, void*);
 /* cusparse.h:5175 -- spmm_csr_batched_example.c:140 (the library has no getter for the strides: the shim records them) */
 B200SPMV_EXPORT cusparseStatus_t cusparseCsrSetStridedBatch(cusparseSpMatDescr_t, int, int64_t, int64_t);
+/* cusparse.h:5170 -- spmm_coo_batched_example.c:137 (one stride for the row, column and value arrays; recorded by the shim) */
+B200SPMV_EXPORT cusparseStatus_t cusparseCooSetStridedBatch(cusparseSpMatDescr_t, int, int64_t);
 /* cusparse.h:5094 / 5100 / 5106 / 5129 -- spmv_csr_example.c:93-95,116-117, cg_example.c:371-378 */
 B200SPMV_EXPORT cusparseStatus_t cusparseCreateDnVec(cusparseDnVecDescr_t*, int64_t, void*, cudaDataType);
 B200SPMV_EXPORT cusparseStatus_t cusparseCreateConstDnVec(cusparseConstDnVecDescr_t*, int64_t, const void*, cudaDataType);
