@@ -23,6 +23,7 @@
 
 #include <type_traits>
 
+#include "mma_sm90.cuh"
 #include "spmv_common.cuh"
 #include "../../include/b200spmv.h"
 
@@ -93,37 +94,6 @@ __global__ void __launch_bounds__(BELL_SC_X * BELL_SC_Y) bell_scalar_kernel(cons
 }
 
 // ------------------------------------------------------------------------------------------------ tensor path
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem, int bytes) {
-    const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(s), "l"(gmem), "r"(bytes));
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-__device__ __forceinline__ void ldsm_x4(const void* p, unsigned (&r)[4]) {
-    const unsigned s = (unsigned)__cvta_generic_to_shared(p);
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(s));
-}
-__device__ __forceinline__ void ldsm_x4_trans(const void* p, unsigned (&r)[4]) {
-    const unsigned s = (unsigned)__cvta_generic_to_shared(p);
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(s));
-}
-
-template <typename T>
-__device__ __forceinline__ void mma16816(float (&c)[4], const unsigned (&a)[4], unsigned b0, unsigned b1) {
-    if constexpr (std::is_same<T, __half>::value)
-        asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                     : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-    else
-        asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                     : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
 template <typename T, int BM, bool BROW>
 __global__ void __launch_bounds__(BELL_THREADS) bell_mma_kernel(const BellArgs a) {
     constexpr int WARPS_M = BM == 16 ? 1 : 2, WARPS_N = 4 / WARPS_M;

@@ -200,6 +200,34 @@ B200SPMV_EXPORT int b200sddmm_csr(void* stream, int dtype, int64_t m, int64_t n,
  * the strided path; a warp steps through its chunk 32 / G * entries_per_group entries at a time. */
 B200SPMV_EXPORT void b200sddmm_params(int32_t* warp_chunk, int32_t* entries_per_group, int32_t* vec_bytes, int32_t* max_group);
 
+/* Sampled dense-dense product for a BSR C (sddmm_bsr.cu): C = alpha * (op(A) * op(B)) o spy(C) + beta * C, C m x n in square
+ * bs x bs blocks (m and n multiples of bs), op(A) m x k and op(B) k x n dense.  Replaces cusparseSDDMM for BSR descriptors
+ * (cuSPARSE/sddmm_bsr/sddmm_bsr_example.c).
+ *   ab_type   : type of A and B: 0 = fp32, 1 = fp64 (cudaDataType CUDA_R_32F / _64F), 2 = fp16, 14 = bf16.
+ *   c_type    : ab_type, or 0 = fp32 for 16-bit A and B.  alpha / beta and the accumulation are fp64 for fp64, fp32 otherwise.
+ *   offsets   : m / bs + 1 int32 block offsets, columns: bnnz int32 block columns, both with index base `base`.
+ *   values    : bnnz blocks of bs * bs values, each row-major (c_row_major = 1) or column-major inside the block.
+ *   A, B      : op(A)(i, k) = A[i * sai + k * sak], op(B)(k, j) = B[k * sbk + j * sbj] (element strides >= 0, as b200sddmm_csr).
+ * batch >= 1 products run in one launch; matrix b uses offsets + b * off_stride, columns + b * col_stride, values + b * val_stride,
+ * A + b * a_stride, B + b * b_stride (elements; 0 = shared; val_stride >= bnnz * bs * bs when batch > 1).
+ * 16-bit A and B with bs % 16 == 0 run on tensor cores (mma.sync, fp32 accumulators) when b200sddmm_bsr_path() says so; fp32 / fp64
+ * and every other 16-bit call run on CUDA cores (FFMA / DFMA).  Each C entry is written once in a fixed k order (no atomics:
+ * identical bits on every call), rounded once to C's type; beta == 0 never reads C; K = 0 gives C = beta * C.  Nothing is read
+ * past K, in ld padding, or in rows / columns of op(A) / op(B) that no stored block references.  No workspace, no allocation, no
+ * host synchronisation. */
+B200SPMV_EXPORT int b200sddmm_bsr(void* stream, int ab_type, int c_type, int64_t m, int64_t n, int64_t k, int64_t bs, int64_t bnnz,
+                                  const void* offsets, const void* columns, void* values, int32_t base, int c_row_major,
+                                  const void* alpha, const void* beta, int scalars_on_device, const void* A, int64_t sai, int64_t sak,
+                                  const void* B, int64_t sbk, int64_t sbj, int batch, int64_t off_stride, int64_t col_stride,
+                                  int64_t val_stride, int64_t a_stride, int64_t b_stride);
+/* 1 when b200sddmm_bsr runs these operands on tensor cores (16-bit, bs % 16 == 0, A and B 16-byte aligned, each operand contiguous
+ * along K or along its other dimension with the other stride and the batch strides multiples of 8), 0 for the CUDA-core kernel. */
+B200SPMV_EXPORT int b200sddmm_bsr_path(int ab_type, int64_t bs, const void* A, int64_t sai, int64_t sak, const void* B, int64_t sbk,
+                                       int64_t sbj, int batch, int64_t a_stride, int64_t b_stride);
+/* sddmm_bsr's constants: K of one tensor-path slab, slabs in flight, the widest block one tensor-path CTA owns whole (a wider block
+ * is split into max_tile x max_tile tiles along its rows and columns, never along K), threads of a CUDA-core CTA. */
+B200SPMV_EXPORT void b200sddmm_bsr_params(int32_t* k_slab, int32_t* stages, int32_t* max_tile, int32_t* fma_threads);
+
 /* The BLAS-1 part of a CG iteration, fused, all scalars in DEVICE memory (no host synchronisation, CUDA-graph capturable).
  * Replaces the cublasDdot / cublasDaxpy / cublasDnrm2 / cublasDscal calls between two cusparseSpMV calls of gpu_CG
  * (cuSPARSE/cg/cg_example.c:226-286).  fp64; vectors 16-byte aligned; `workspace` = b200cg_workspace_bytes() bytes, zeroed
@@ -301,6 +329,12 @@ B200SPMV_EXPORT int b200spmm_batch_count(const void* matA, const void* matB, con
  * B200SPMV_FORWARD=1, and where the closed library measured faster: fp64, and fp32 with K > 32 when op(B) is K-contiguous),
  * 1 = one product on sddmm_csr_kernel, N = a strided batch of N.  Host logic only. */
 B200SPMV_EXPORT int b200sddmm_route(const void* matA, const void* matB, const void* matC, int opA, int opB, int computeType);
+/* Where cusparseSDDMM_bufferSize / _preprocess / cusparseSDDMM send a call with a BSR matC created through the shim: 0 = the closed
+ * library, N >= 1 = N products on b200sddmm_bsr.  Native needs op NON_TRANSPOSE or TRANSPOSE, int32 indices, square blocks, A, B and
+ * C of one real type (or 16-bit A and B with an fp32 C) with a compute type of fp32 (fp64 for fp64), a batch layout the closed
+ * library accepts, no B200SPMV_FORWARD=1, and a class measured at least at parity with the closed library (DESIGN.md 3.16).  A BSR
+ * descriptor created behind the shim's back is forwarded.  Host logic only. */
+B200SPMV_EXPORT int b200sddmm_bsr_route(const void* matA, const void* matB, const void* matC, int opA, int opB, int computeType);
 /* Where cusparseSpMM sends a call with a Blocked-ELL matA (descriptors passed as void*, enum values as int): 1 = b200spmm_bell,
  * 0 = the closed library.  Native needs NON_TRANSPOSE for both operands, alg DEFAULT or BLOCKED_ELL_ALG1, int32 block columns,
  * fp16 / bf16 A and B of one type, C of that type or fp32, compute type fp32, no strided batch, rows and cols multiples of the
@@ -366,6 +400,15 @@ B200SPMV_EXPORT cusparseStatus_t cusparseSpMatSetValues(cusparseSpMatDescr_t, vo
 B200SPMV_EXPORT cusparseStatus_t cusparseCsrSetStridedBatch(cusparseSpMatDescr_t, int, int64_t, int64_t);
 /* cusparse.h:5170 -- spmm_coo_batched_example.c:137 (one stride for the row, column and value arrays; recorded by the shim) */
 B200SPMV_EXPORT cusparseStatus_t cusparseCooSetStridedBatch(cusparseSpMatDescr_t, int, int64_t);
+/* cusparse.h:5327 / 5343 / 5181 -- sddmm_bsr_example.c (the library has no BSR getter: the shim records block size, block order
+ * and the three batch strides) */
+B200SPMV_EXPORT cusparseStatus_t cusparseCreateBsr(cusparseSpMatDescr_t*, int64_t, int64_t, int64_t, int64_t, int64_t, void*, void*,
+                                                   void*, cusparseIndexType_t, cusparseIndexType_t, cusparseIndexBase_t, cudaDataType,
+                                                   cusparseOrder_t);
+B200SPMV_EXPORT cusparseStatus_t cusparseCreateConstBsr(cusparseConstSpMatDescr_t*, int64_t, int64_t, int64_t, int64_t, int64_t,
+                                                        const void*, const void*, const void*, cusparseIndexType_t,
+                                                        cusparseIndexType_t, cusparseIndexBase_t, cudaDataType, cusparseOrder_t);
+B200SPMV_EXPORT cusparseStatus_t cusparseBsrSetStridedBatch(cusparseSpMatDescr_t, int, int64_t, int64_t, int64_t);
 /* cusparse.h:5094 / 5100 / 5106 / 5129 -- spmv_csr_example.c:93-95,116-117, cg_example.c:371-378 */
 B200SPMV_EXPORT cusparseStatus_t cusparseCreateDnVec(cusparseDnVecDescr_t*, int64_t, void*, cudaDataType);
 B200SPMV_EXPORT cusparseStatus_t cusparseCreateConstDnVec(cusparseConstDnVecDescr_t*, int64_t, const void*, cudaDataType);
