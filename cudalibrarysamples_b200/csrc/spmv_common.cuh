@@ -45,6 +45,40 @@ __device__ __forceinline__ float ldg_stream(const float* p) {
     return r;
 }
 
+// ---- cold x gathers of csr_flat_kernel with a hot plan: columns outside the packed hot set (spmv_csr_flat.cu).
+//      B200_FLAT_COLD picks how they treat L1: 0 = like the hot gather (read-only path, allocating), 1 = L1::evict_first,
+//      2 = .cg (L2 only: cold lines never displace the packed hot lines).  2 was fastest on the H100 and 1 slowest
+//      (DESIGN.md §3.2, scripts/sweep.py flat_l1).  Not L1::no_allocate: its SASS (LDG.E.NA) is that of the val[] stream. ----
+#ifndef B200_FLAT_COLD
+#define B200_FLAT_COLD 2
+#endif
+__device__ __forceinline__ double ldg_cold(const double* p) {
+#if B200_FLAT_COLD == 1
+    double r;
+    asm volatile("ld.global.nc.L1::evict_first.f64 %0, [%1];" : "=d"(r) : "l"(p));
+    return r;
+#elif B200_FLAT_COLD == 2
+    double r;
+    asm volatile("ld.global.cg.f64 %0, [%1];" : "=d"(r) : "l"(p));
+    return r;
+#else
+    return __ldg(p);
+#endif
+}
+__device__ __forceinline__ float ldg_cold(const float* p) {
+#if B200_FLAT_COLD == 1
+    float r;
+    asm volatile("ld.global.nc.L1::evict_first.f32 %0, [%1];" : "=f"(r) : "l"(p));
+    return r;
+#elif B200_FLAT_COLD == 2
+    float r;
+    asm volatile("ld.global.cg.f32 %0, [%1];" : "=f"(r) : "l"(p));
+    return r;
+#else
+    return __ldg(p);
+#endif
+}
+
 // 4 consecutive values starting at a 16-byte-aligned element index.
 __device__ __forceinline__ void load4_stream(const double* p, double (&v)[4]) {
     double2 a = ldg_stream_v2(p), b = ldg_stream_v2(p + 2);

@@ -72,9 +72,12 @@ static_assert(FLAT_STEPS % FLAT_BATCH64 == 0 && FLAT_STEPS % FLAT_BATCH32 == 0, 
 
 // Hot columns of x.  Preprocess picks the most-used columns whose values fit B200_FLAT_HOT_BYTES, and every SpMV first packs
 // their x values densely (xh) so the gather of csr_flat_kernel finds them on fewer, fully used cache lines.  On R-MAT the
-// hot columns are scattered over lines shared with cold columns; packed, more of the gathers hit L1.
+// hot columns are scattered over lines shared with cold columns; packed, more of the gathers hit L1.  With a hot plan the
+// cold gathers go to L2 only (ldg_cold, spmv_common.cuh): when they allocated L1 lines, their stream (about half the
+// gathers of R-MAT 1 M, nearly all on distinct lines) evicted packed lines before their next use, so a budget beyond 64 KB
+// bought pack traffic and no hits.  With the cold gathers out of L1, budgets up to about 128 KB gain.
 #ifndef B200_FLAT_HOT_BYTES
-#define B200_FLAT_HOT_BYTES (64 * 1024)   // swept over 0 / 64 / 96 / 128 / 160 KB on the H100: scripts/sweep.py flat_hot
+#define B200_FLAT_HOT_BYTES (128 * 1024)  // swept over 0 ... 192 KB with each cold-gather policy on the H100: scripts/sweep.py flat_l1
 #endif
 constexpr int HOT_BYTES = B200_FLAT_HOT_BYTES;
 constexpr int HOT_MAX = HOT_BYTES / 4;              // slots of the hot list: fp32 fits twice as many values as fp64
@@ -357,7 +360,9 @@ __device__ __forceinline__ void flat_store_y(T* yp, T alpha, T v, T beta) {
     *yp = alpha * v + beta * old;
 }
 
-template <typename T>
+// HOT: the matrix has a hot plan (col is colp).  Only then do the cold gathers take the ldg_cold policy: without packed hot
+// lines to protect, every gather is "cold", and keeping them all out of L1 loses every L1 hit (DESIGN.md §3.2, 0 KB row).
+template <typename T, bool HOT>
 __global__ void __launch_bounds__(FLAT_BLOCK, B200_FLAT_MIN_CTAS) csr_flat_kernel(const FlatArgs<T> a) {
     __shared__ T   sFirst[FLAT_WARPS], sLast[FLAT_WARPS];
     __shared__ int sFrow[FLAT_WARPS];                      // >= 0: row of the chunk's first row end (deferred to the stitch)
@@ -410,7 +415,9 @@ __global__ void __launch_bounds__(FLAT_BLOCK, B200_FLAT_MIN_CTAS) csr_flat_kerne
             T p[FLAT_BATCH];
 #pragma unroll
             for (int k = 0; k < FLAT_BATCH; k++)
-                p[k] = (n0 + (kb + k) * 32 + lane < n1) ? vv[k] * (cc[k] < 0 ? __ldg(a.xh + ~cc[k]) : __ldg(xp + cc[k])) : T(0);
+                p[k] = (n0 + (kb + k) * 32 + lane < n1)
+                           ? vv[k] * (HOT && cc[k] < 0 ? __ldg(a.xh + ~cc[k]) : HOT ? ldg_cold(xp + cc[k]) : __ldg(xp + cc[k]))
+                           : T(0);
             if (kb + FLAT_BATCH < FLAT_STEPS && n0 + (kb + FLAT_BATCH) * 32 < n1) issue(kb + FLAT_BATCH);
 #pragma unroll
             for (int k = 0; k < FLAT_BATCH; k++) {
@@ -553,7 +560,8 @@ static int launch_flat(cudaStream_t stream, int64_t rows, int64_t nnz, const voi
         a.base = 0;
     }
     const int64_t nctas = flat_num_ctas(nnz);
-    csr_flat_kernel<T><<<(unsigned)nctas, FLAT_BLOCK, 0, stream>>>(a);
+    if (nhot > 0) csr_flat_kernel<T, true><<<(unsigned)nctas, FLAT_BLOCK, 0, stream>>>(a);
+    else          csr_flat_kernel<T, false><<<(unsigned)nctas, FLAT_BLOCK, 0, stream>>>(a);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return (int)e;
     // empty rows + CTA-crossing rows; with a host-side beta == 1 the empty rows need no pass at all

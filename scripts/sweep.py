@@ -8,6 +8,7 @@ Variants are -D overrides of the tunables at the top of csrc/spmv_csr.cu.
 """
 import json
 import os
+import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -110,6 +111,9 @@ if os.environ.get("SWEEP_SET") == "flat4":
 if os.environ.get("SWEEP_SET") == "flat_hot":
     # csr_flat_kernel: byte budget of the packed hot columns of x (0 = no hot plan)
     VARIANTS = {f"flat_hot{kb}k": dict(FLATHOT=kb) for kb in (0, 64, 96, 128, 160)}
+if os.environ.get("SWEEP_SET") == "flat_l1":
+    # csr_flat_kernel: (B200_FLAT_COLD = L1 policy of the cold x gathers, hot budget in KB); run with SWEEP_ROUNDS=3
+    VARIANTS = {f"flat_l1_p{p}_h{kb}k": dict(FLATL1=(p, kb)) for p in (0, 1, 2) for kb in (0, 64, 96, 128, 160, 192)}
 if os.environ.get("SWEEP_SET") == "short":
     # csr_short_kernel: (warps per CTA, load steps per pass, resident CTAs)
     VARIANTS = {f"short_w{w}_s{st}_occ{o}": dict(SHORT=(w, st, o)) for (w, st, o) in
@@ -126,6 +130,9 @@ def flags(v):
         return [f"-DB200_FLAT_QUIET_BALLOT={v['FLAT3'][0]}", f"-DB200_FLAT_EMPTY_TAIL={v['FLAT3'][1]}"]
     if "FLATHOT" in v:
         return [f"-DB200_FLAT_HOT_BYTES={v['FLATHOT'] * 1024}"]
+    if "FLATL1" in v:
+        p, kb = v["FLATL1"]
+        return [f"-DB200_FLAT_COLD={p}", f"-DB200_FLAT_HOT_BYTES={kb * 1024}"]
     if "SHORT" in v:
         w, st, o = v["SHORT"]
         return [f"-DB200_SHORT_WARPS={w}", f"-DB200_SHORT_STEPS={st}", f"-DB200_SHORT_MIN_CTAS={o}"]
@@ -151,14 +158,38 @@ def flags(v):
             f"-DB200_CSR_BATCH={v['BATCH']}", f"-DB200_CSR_MIN_CTAS={v['MIN']}"]
 
 
+def build_flat_only(b, tag, extra, out):
+    """The csr_flat_kernel tunables are read by spmv_csr_flat.cu alone: compile that file, link it with the default build's
+    objects of every other file."""
+    bdir = os.path.join(b.PKG_DIR, "build", "v_" + tag)
+    os.makedirs(bdir, exist_ok=True)
+    obj = os.path.join(bdir, "spmv_csr_flat.cu.o")
+    cmd = [b.nvcc(), *b.NVCC_FLAGS, *extra, "-c", os.path.join(b.CSRC, "spmv_csr_flat.cu"), "-o", obj]
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    with open(os.path.join(bdir, "build.log"), "w") as f:
+        f.write("$ " + " ".join(cmd) + "\n" + r.stdout + r.stderr)
+    if r.returncode != 0:
+        raise RuntimeError(f"nvcc failed on variant {tag}:\n{r.stdout}{r.stderr}")
+    objs = [obj if s == "spmv_csr_flat.cu" else os.path.join(b.PKG_DIR, "build", s + ".o") for s in b.SOURCES]
+    subprocess.run([b.nvcc(), "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", out, *objs, "-ldl", "-lpthread"], check=True)
+
+
 def build():
+    from concurrent.futures import ThreadPoolExecutor
     from cudalibrarysamples_b200 import build as b
     os.makedirs(VDIR, exist_ok=True)
+    flat_only = {t: v for t, v in VARIANTS.items() if "FLATL1" in v}
+    if flat_only:
+        b.build_native()                                        # the objects the flat-only variants link against
+        with ThreadPoolExecutor(os.cpu_count() or 4) as ex:
+            list(ex.map(lambda tv: build_flat_only(b, tv[0], flags(tv[1]), os.path.join(VDIR, f"libb200spmv_{tv[0]}.so")),
+                        flat_only.items()))
     for tag, v in VARIANTS.items():
         out = os.path.join(VDIR, f"libb200spmv_{tag}.so")
-        b.build_native(extra_flags=flags(v), out_path=out, tag="v_" + tag)
+        if tag not in flat_only:
+            b.build_native(extra_flags=flags(v), out_path=out, tag="v_" + tag)
         log = open(os.path.join(ROOT, "cudalibrarysamples_b200", "build", "v_" + tag, "build.log")).read()
-        i = log.find("csr_short_kernelIdEE") if "SHORT" in v else log.find("csr_flat_kernelIdEE") if ("FLAT" in v or "FLAT3" in v or "FLATHOT" in v) else log.find("csr_seg_kernelIdEE") if "SEG" in v else log.find("csr_rowwise_kernelIdEE") if "RW" in v else log.find("csr_ws_kernelIdEE") if "WS" in v else max(log.find("csr_pipe_kernelIdEE"), log.find("csr_tile_kernelIdEE")) if "-DB200_CSR_KERNEL=0" not in " ".join(flags(v)) else log.find("csr_tile_kernelIdEE")
+        i = log.find("csr_short_kernelIdEE") if "SHORT" in v else log.find("csr_flat_kernelIdEE") if ("FLAT" in v or "FLAT3" in v or "FLATHOT" in v or "FLATL1" in v) else log.find("csr_seg_kernelIdEE") if "SEG" in v else log.find("csr_rowwise_kernelIdEE") if "RW" in v else log.find("csr_ws_kernelIdEE") if "WS" in v else max(log.find("csr_pipe_kernelIdEE"), log.find("csr_tile_kernelIdEE")) if "-DB200_CSR_KERNEL=0" not in " ".join(flags(v)) else log.find("csr_tile_kernelIdEE")
         regs = log[i:i + 400].split("Used ")[1].split(",")[0] if i >= 0 else "?"
         print(tag, regs)
 
@@ -207,7 +238,11 @@ def run(workloads, variants=None, steps=100):
         nbytes = W.csr_bytes(rows, rows, nnz, val.element_size())
         ref = None
         print(f"== {wl}: rows={rows} nnz={nnz} alg_bytes={nbytes / 1e6:.1f} MB", flush=True)
-        for tag, path in libs + [("cusparse", "closed")]:
+        order = libs + [("cusparse", "closed")]
+        # SWEEP_ROUNDS > 1: the whole list again, every other round in reverse order, so that drift of the clock or of the
+        # neighbours' load spreads over all variants; results then hold one entry per round
+        rounds = int(os.environ.get("SWEEP_ROUNDS", "1"))
+        for tag, path in [tp for r in range(rounds) for tp in (order if r % 2 == 0 else order[::-1])]:
             api = cs.Api("cusparse") if tag == "cusparse" else cs.Api("b200", lib_path=path)
             if tag != "cusparse":
                 parts = tag.split(":") if tag.startswith("kernel:") else ["", "auto"]
@@ -230,8 +265,13 @@ def run(workloads, variants=None, steps=100):
             if ref is None:
                 ref = y.clone()
             err = float((torch.linalg.norm(y.double() - ref.double()) / torch.linalg.norm(ref.double())).item())
-            print(f"  {tag:24s} {us:9.2f} us  {nbytes / us / 1e3:8.1f} GB/s  relerr_vs_first {err:.1e}", flush=True)
-            results.setdefault(wl, {})[tag] = dict(us=us, gbs=nbytes / us / 1e3, err=err)
+            same = bool(torch.equal(y, ref))
+            print(f"  {tag:24s} {us:9.2f} us  {nbytes / us / 1e3:8.1f} GB/s  relerr_vs_first {err:.1e}  bits_equal {same}", flush=True)
+            r = dict(us=us, gbs=nbytes / us / 1e3, err=err, bits_equal=same)
+            if rounds > 1:
+                results.setdefault(wl, {}).setdefault(tag, []).append(r)
+            else:
+                results.setdefault(wl, {})[tag] = r
             op.close()
         del off, col, val, x
         torch.cuda.empty_cache()
