@@ -19,6 +19,15 @@ void* open_real_cusparse(const char* tag) {
     abort();
 }
 
+void* real_symbol(void* h, const char* name, const char* tag) {
+    void* f = dlsym(h, name);
+    if (!f) {
+        fprintf(stderr, "[%s] FATAL: real libcusparse lacks %s\n", tag, name);
+        abort();
+    }
+    return f;
+}
+
 bool env_flag(const char* name) {
     const char* v = getenv(name);
     return v && v[0] && v[0] != '0';

@@ -11,7 +11,6 @@
 // every call under B200SPMV_FORWARD=1.  B200SPMV_LOG=1 names the path of each call on stderr.
 #include <cuda_runtime_api.h>
 #include <cusparse.h>
-#include <dlfcn.h>
 
 #include <atomic>
 #include <cstdio>
@@ -24,22 +23,17 @@
 
 namespace {
 
+// Every real-library function this shim calls: expanded into the members of Real and into their loads.
+#define SPSV_REAL_FNS(X)                                                                                                      \
+    X(cusparseSpSV_createDescr) X(cusparseSpSV_destroyDescr) X(cusparseSpSV_bufferSize) X(cusparseSpSV_analysis)             \
+    X(cusparseSpSV_solve) X(cusparseSpSV_updateMatrix) X(cusparseGetStream) X(cusparseGetPointerMode) X(cusparseSpMatGetFormat) \
+    X(cusparseSpMatGetAttribute) X(cusparseConstCsrGet) X(cusparseConstDnVecGet)
+
 struct Real {
     void* h = nullptr;
-#define REAL_FN(name) decltype(&::name) name = nullptr;
-    REAL_FN(cusparseSpSV_createDescr)
-    REAL_FN(cusparseSpSV_destroyDescr)
-    REAL_FN(cusparseSpSV_bufferSize)
-    REAL_FN(cusparseSpSV_analysis)
-    REAL_FN(cusparseSpSV_solve)
-    REAL_FN(cusparseSpSV_updateMatrix)
-    REAL_FN(cusparseGetStream)
-    REAL_FN(cusparseGetPointerMode)
-    REAL_FN(cusparseSpMatGetFormat)
-    REAL_FN(cusparseSpMatGetAttribute)
-    REAL_FN(cusparseConstCsrGet)
-    REAL_FN(cusparseConstDnVecGet)
-#undef REAL_FN
+#define REAL_MEMBER(name) decltype(&::name) name = nullptr;
+    SPSV_REAL_FNS(REAL_MEMBER)
+#undef REAL_MEMBER
     bool forward = false, log = false;
 };
 
@@ -51,13 +45,9 @@ void init_real() {
     r->forward = b200::env_flag("B200SPMV_FORWARD");
     r->log = b200::env_flag("B200SPMV_LOG");
     r->h = b200::open_real_cusparse("b200spsv");
-#define LOAD(name)                                                                                   \
-    r->name = (decltype(r->name))dlsym(r->h, #name);                                                 \
-    if (!r->name) { fprintf(stderr, "[b200spsv] FATAL: real libcusparse lacks %s\n", #name); abort(); }
-    LOAD(cusparseSpSV_createDescr) LOAD(cusparseSpSV_destroyDescr) LOAD(cusparseSpSV_bufferSize) LOAD(cusparseSpSV_analysis)
-    LOAD(cusparseSpSV_solve) LOAD(cusparseSpSV_updateMatrix) LOAD(cusparseGetStream) LOAD(cusparseGetPointerMode)
-    LOAD(cusparseSpMatGetFormat) LOAD(cusparseSpMatGetAttribute) LOAD(cusparseConstCsrGet) LOAD(cusparseConstDnVecGet)
-#undef LOAD
+#define REAL_LOAD(name) r->name = (decltype(r->name))b200::real_symbol(r->h, #name, "b200spsv");
+    SPSV_REAL_FNS(REAL_LOAD)
+#undef REAL_LOAD
     g_real = r;
 }
 

@@ -1,15 +1,16 @@
 #!/bin/bash
-# Host-side memory / UB check of the shim without a GPU: cusparse_shim.cpp + config.cpp compiled with
+# Host-side memory / UB check of the shim without a GPU: cusparse_shim.cpp + config.cpp + real_cusparse.cpp compiled with
 # -fsanitize=address,undefined, linked with the library's ordinary CUDA objects (cudalibrarysamples_b200/build/*.cu.o, built by
 # __graft_entry__.build()), then the descriptor / routing script of tests/test_descriptors_cpu.py is run against that build.
 # Round 2: clean ("OK", no sanitizer report).
 set -e
 cd "$(dirname "$0")/../cudalibrarysamples_b200"
 mkdir -p build/asan
-for f in cusparse_shim config; do
+for f in cusparse_shim config real_cusparse; do
   g++ -O1 -g -std=c++17 -fPIC -fsanitize=address,undefined -fno-omit-frame-pointer -w -I/usr/local/cuda/include -c csrc/$f.cpp -o build/asan/$f.o
 done
-g++ -shared -fsanitize=address,undefined -o build/asan/libb200spmv_asan.so build/asan/cusparse_shim.o build/asan/config.o build/*.cu.o \
+g++ -shared -fsanitize=address,undefined -o build/asan/libb200spmv_asan.so build/asan/cusparse_shim.o build/asan/config.o \
+    build/asan/real_cusparse.o build/*.cu.o \
     -L/usr/local/cuda/lib64 -lcudart -ldl -lpthread
 cd ..
 python - <<'PY'

@@ -98,6 +98,63 @@ SCRIPT = textwrap.dedent("""
     for d in (A, A1, A2):
         assert shim.cusparseDestroySpMat(d) == 0
     assert real.cusparseDestroySpMat(A3) == 0
+    # cusparseCreateX and cusparseCreateConstX through the shim, for every kind it records: the real getters see the same values, and
+    # the route exports give both the same (native) answer -- a BSR descriptor the shim did not record would be forwarded
+    I64, VP, INT = C.c_int64, C.c_void_p, C.c_int
+    F16, ROW, NT, TR = 2, 2, 0, 1
+    shim.b200sddmm_route.argtypes = shim.b200sddmm_bsr_route.argtypes = [C.c_void_p] * 3 + [C.c_int] * 3
+    shim.b200spmm_coo_route.argtypes = [C.c_void_p] * 3 + [C.c_int] * 4
+    big = (C.c_double * (1 << 20))()
+    at = C.addressof
+
+    def both(kind, *args):
+        made = []
+        for f in ("cusparseCreate" + kind, "cusparseCreateConst" + kind):
+            d = C.c_void_p()
+            assert getattr(shim, f)(C.byref(d), *args) == 0, f
+            made.append(d)
+        return made
+
+    def get(fn, d, *types):
+        out = [t() for t in types]
+        assert getattr(real, fn)(d, *[C.byref(o) for o in out]) == 0, fn
+        return [o.value for o in out]
+
+    def spmat(d):                                          # what every sparse descriptor answers (no Sliced-ELL / BSR getter exists)
+        return (get("cusparseSpMatGetFormat", d, INT) + get("cusparseSpMatGetSize", d, I64, I64, I64) +
+                get("cusparseSpMatGetIndexBase", d, INT) + get("cusparseConstSpMatGetValues", d, VP))
+
+    def dnm(r, c_, vt, order):
+        d = C.c_void_p()
+        assert real.cusparseCreateDnMat(C.byref(d), C.c_int64(r), C.c_int64(c_), C.c_int64(c_ if order == ROW else r), big, vt, order) == 0
+        return d
+
+    made = []
+    pair = both("Csr", C.c_int64(4), C.c_int64(3), C.c_int64(4), off, col, val, I32, I32, 1, F32)
+    for d in pair:
+        csr_seen = get("cusparseConstCsrGet", d, I64, I64, I64, VP, VP, VP, INT, INT, INT, INT)
+        assert csr_seen == [4, 3, 4, at(off), at(col), at(val), I32, I32, 1, F32]
+        assert shim.b200sddmm_route(dnm(4, 5, F32, ROW), dnm(5, 3, F32, ROW), d, NT, NT, F32) == 1
+    made += pair
+    M = 1 << 16
+    pair = both("Coo", C.c_int64(M), C.c_int64(48), C.c_int64(16 * M), off, col, val, I32, 0, F32)
+    for d in pair:
+        assert get("cusparseConstCooGet", d, I64, I64, I64, VP, VP, VP, INT, INT, INT) == [M, 48, 16 * M, at(off), at(col), at(val), I32, 0, F32]
+        assert shim.b200spmm_coo_route(d, dnm(48, 32, F32, COL), dnm(M, 32, F32, COL), NT, NT, F32, 0) == 1
+    made += pair
+    pair = both("SlicedEll", C.c_int64(4), C.c_int64(4), C.c_int64(9), C.c_int64(12), C.c_int64(2), off, col, val, I32, I32, 0, F32)
+    assert spmat(pair[0]) == spmat(pair[1]) == [7, 4, 4, 9, 0, at(val)]
+    made += pair
+    pair = both("Bsr", C.c_int64(256), C.c_int64(256), C.c_int64(64), C.c_int64(16), C.c_int64(16), off, col, big, I32, I32, 0, F16, ROW)
+    assert spmat(pair[0]) == spmat(pair[1]) and spmat(pair[0])[0] == 6 and spmat(pair[0])[-1] == at(big)
+    for d in pair:
+        assert shim.b200sddmm_bsr_route(dnm(4096, 64, F16, ROW), dnm(4096, 64, F16, ROW), d, NT, TR, F32) == 1
+    made += pair
+    for d in made:
+        assert shim.cusparseDestroySpMat(d) == 0
+    for d in both("DnVec", C.c_int64(24), B, F32):
+        assert get("cusparseConstDnVecGet", d, I64, VP, INT) == [24, at(B), F32]
+        assert shim.cusparseDestroyDnVec(d) == 0
     print("OK")
 """)
 
