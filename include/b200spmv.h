@@ -228,6 +228,39 @@ B200SPMV_EXPORT int b200sddmm_bsr_path(int ab_type, int64_t bs, const void* A, i
  * is split into max_tile x max_tile tiles along its rows and columns, never along K), threads of a CUDA-core CTA. */
 B200SPMV_EXPORT void b200sddmm_bsr_params(int32_t* k_slab, int32_t* stages, int32_t* max_tile, int32_t* fma_threads);
 
+/* BSR x dense (spmm_bsr.cu): C = alpha * A * op(B) + beta * C, A m x k in square bs x bs blocks (m and k multiples of bs), op(B)
+ * k x n and C m x n dense.  Replaces cusparseSpMM for BSR descriptors: the P . V of block-sparse attention.
+ *   ab_type   : type of A's values and of B: 0 = fp32, 1 = fp64, 2 = fp16, 14 = bf16 (cudaDataType).
+ *   c_type    : ab_type, or 0 = fp32 for 16-bit A and B.  alpha / beta and the accumulation are fp64 for fp64, fp32 otherwise.
+ *   offsets   : m / bs + 1 int32 block offsets, columns: bnnz int32 block columns, both with index base `base`.
+ *   values    : bnnz blocks of bs * bs values, each row-major (a_row_major = 1) or column-major inside the block.
+ *   B         : op(B)(k, j) = B[k * sbk + j * sbj] (element strides >= 0, as b200sddmm_bsr).
+ *   C         : row- or column-major with leading dimension ldc (elements).
+ * batch >= 1 products run in one launch; matrix b uses offsets + b * off_stride, columns + b * col_stride, values + b * val_stride,
+ * B + b * b_stride, C + b * c_stride (elements; 0 = shared, except C, whose matrices must not overlap).
+ *   workspace : b200spmm_bsr_workspace_bytes() bytes, 16-byte aligned: carry slots that let a long block-row be split over several
+ *               CTAs.  A NULL, misaligned or smaller buffer runs one CTA per block-row; both give identical bits.
+ * 16-bit A and B with bs % 16 == 0 run on tensor cores (mma.sync, fp32 accumulators) when b200spmm_bsr_path() says so; fp32 / fp64
+ * and every other call on CUDA cores (FFMA / DFMA).  Each C entry is written once in a fixed order (no atomics: identical bits on
+ * every call); beta == 0 never reads C; block-rows that store nothing get beta * C.  Nothing is read past n, in ld padding, or in
+ * rows of op(B) no stored block references.  No allocation, no host synchronisation. */
+B200SPMV_EXPORT int b200spmm_bsr(void* stream, int ab_type, int c_type, int64_t m, int64_t k, int64_t n, int64_t bs, int64_t bnnz,
+                                 const void* offsets, const void* columns, const void* values, int32_t base, int a_row_major,
+                                 const void* alpha, const void* beta, int scalars_on_device, const void* B, int64_t sbk, int64_t sbj,
+                                 void* C, int64_t ldc, int c_row_major, int batch, int64_t off_stride, int64_t col_stride,
+                                 int64_t val_stride, int64_t b_stride, int64_t c_stride, void* workspace, size_t workspace_bytes);
+B200SPMV_EXPORT size_t b200spmm_bsr_workspace_bytes(int ab_type, int64_t m, int64_t n, int64_t bs, int64_t bnnz, int batch);
+/* 1 when b200spmm_bsr runs these operands on tensor cores (16-bit, bs % 16 == 0, row-major blocks, values and B 16-byte aligned,
+ * op(B) contiguous along K or N with the other stride and the batch strides multiples of 8), 0 for the CUDA-core kernel. */
+B200SPMV_EXPORT int b200spmm_bsr_path(int ab_type, int64_t bs, int a_row_major, const void* values, const void* B, int64_t sbk,
+                                      int64_t sbj, int batch, int64_t val_stride, int64_t b_stride);
+/* spmm_bsr's constants: K of one tensor-path slab, slabs per pipeline stage, stages in flight, the most rows of a block-row one
+ * tensor-path CTA owns, and the piece length: a block-row is cut into pieces of ch = max(chunk_min, min(ceil(chunk_factor * bnnz /
+ * (m / bs)), ceil(bnnz * batch * ceil(bs / 64) * ceil(n / 128) / target_ctas))) stored blocks, and with a workspace CTA c walks the
+ * pieces that start in stored blocks [c * ch, (c + 1) * ch). */
+B200SPMV_EXPORT void b200spmm_bsr_params(int32_t* k_slab, int32_t* slabs_per_stage, int32_t* stages, int32_t* max_rows_per_cta,
+                                         int32_t* chunk_min, int32_t* chunk_factor, int32_t* target_ctas);
+
 /* The BLAS-1 part of a CG iteration, fused, all scalars in DEVICE memory (no host synchronisation, CUDA-graph capturable).
  * Replaces the cublasDdot / cublasDaxpy / cublasDnrm2 / cublasDscal calls between two cusparseSpMV calls of gpu_CG
  * (cuSPARSE/cg/cg_example.c:226-286).  fp64; vectors 16-byte aligned; `workspace` = b200cg_workspace_bytes() bytes, zeroed
@@ -348,6 +381,13 @@ B200SPMV_EXPORT int b200spmm_bell_route(const void* matA, const void* matB, cons
  * B200SPMV_FORWARD=1, and a class measured at least at parity with the closed library (DESIGN.md 3.15).  A shape mismatch stays
  * native: the call rejects it.  Host logic only. */
 B200SPMV_EXPORT int b200spmm_coo_route(const void* matA, const void* matB, const void* matC, int opA, int opB, int computeType, int alg);
+/* Where cusparseSpMM_bufferSize / _preprocess / cusparseSpMM send a call with a BSR matA created through the shim (descriptors passed
+ * as void*, enum values as int): 0 = the closed library, N >= 1 = N products on b200spmm_bsr (a strided batch when N > 1).  Native
+ * needs opA NON_TRANSPOSE, opB NON_TRANSPOSE or TRANSPOSE, alg DEFAULT or BSR_ALG1, int32 indices, square blocks, A and B of one
+ * type with C of that type (or 16-bit A and B with an fp32 C) and a compute type of fp32 (fp64 for fp64), a batch layout the closed
+ * library accepts, no B200SPMV_FORWARD=1, and a class measured at least at parity with the closed library (DESIGN.md 3.17).  A shape
+ * mismatch stays native: the call rejects it.  Host logic only. */
+B200SPMV_EXPORT int b200spmm_bsr_route(const void* matA, const void* matB, const void* matC, int opA, int opB, int computeType, int alg);
 /* name of the main kernel the most recent CSR SpMV launched, e.g. "b200::csr_seg_kernel<double>" (bench.py's roofline.kernel) */
 B200SPMV_EXPORT const char* b200spmv_last_csr_kernel(void);
 
