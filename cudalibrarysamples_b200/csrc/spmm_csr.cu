@@ -119,26 +119,7 @@ __global__ void __launch_bounds__(32 * SPMM_WARPS) spmm_csr_ctile_kernel(const S
     }
 }
 
-// B (cols x n, column-major, leading dimension ldb) -> Bt (cols x n, row-major, tight): 32 x 32 tiles through shared memory
-template <typename T>
-__global__ void __launch_bounds__(256) spmm_transpose_b_kernel(const T* __restrict__ B, long long ldb, T* __restrict__ Bt, int cols, int n) {
-    __shared__ T tile[32][33];
-    const int tx = (int)threadIdx.x & 31, ty = (int)threadIdx.x >> 5;
-    const int k0 = blockIdx.x * 32, j0 = blockIdx.y * 32;
-#pragma unroll
-    for (int i = 0; i < 32; i += 8) {
-        const int k = k0 + tx, j = j0 + ty + i;
-        if (k < cols && j < n) tile[ty + i][tx] = B[(long long)j * ldb + k];
-    }
-    __syncthreads();
-#pragma unroll
-    for (int i = 0; i < 32; i += 8) {
-        const int k = k0 + ty + i, j = j0 + tx;
-        if (k < cols && j < n) Bt[(long long)k * n + j] = tile[tx][ty + i];
-    }
-}
-
-// The same transpose as a host call on `stream` (dtype 0 = fp32, 1 = fp64): sddmm_csr.cu uses it to make an operand K-contiguous.
+// The transpose of spmm_transpose_b_kernel (spmv_common.cuh) as a host call on `stream` (dtype 0 = fp32, 1 = fp64): sddmm_csr.cu uses it to make an operand K-contiguous.
 int transpose_col_to_row_major(cudaStream_t stream, int dtype, const void* B, int64_t ldb, void* Bt, int64_t cols, int64_t n) {
     const dim3 tg((unsigned)((cols + 31) / 32), (unsigned)((n + 31) / 32));
     if (dtype == 1) spmm_transpose_b_kernel<double><<<tg, 256, 0, stream>>>((const double*)B, (long long)ldb, (double*)Bt, (int)cols, (int)n);

@@ -106,6 +106,26 @@ __device__ __forceinline__ T axpby(T alpha, T sum, T beta, const T* y) {
     return beta == T(0) ? alpha * sum : alpha * sum + beta * (*y);
 }
 
+// B (cols x n, column-major, leading dimension ldb) -> Bt (cols x n, row-major, tight): 32 x 32 tiles through shared memory.
+// The row-major copy of a column-major B that spmm_csr.cu (fp32 / fp64) and spmm_csr16.cu (fp16 / bf16) read from the workspace.
+template <typename T>
+__global__ void __launch_bounds__(256) spmm_transpose_b_kernel(const T* __restrict__ B, long long ldb, T* __restrict__ Bt, int cols, int n) {
+    __shared__ T tile[32][33];
+    const int tx = (int)threadIdx.x & 31, ty = (int)threadIdx.x >> 5;
+    const int k0 = blockIdx.x * 32, j0 = blockIdx.y * 32;
+#pragma unroll
+    for (int i = 0; i < 32; i += 8) {
+        const int k = k0 + tx, j = j0 + ty + i;
+        if (k < cols && j < n) tile[ty + i][tx] = B[(long long)j * ldb + k];
+    }
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < 32; i += 8) {
+        const int k = k0 + ty + i, j = j0 + tx;
+        if (k < cols && j < n) Bt[(long long)k * n + j] = tile[tx][ty + i];
+    }
+}
+
 template <typename T>
 __device__ __forceinline__ T warp_sum(T v) {
 #pragma unroll

@@ -102,6 +102,12 @@ def shim(build_if_missing: bool = False) -> C.CDLL:
         lib.b200spmm_bsr_workspace_bytes.restype = C.c_size_t
         lib.b200spmm_bsr_path.argtypes = [C.c_int, i64, C.c_int, vp, vp, i64, i64, C.c_int, i64, i64]
         lib.b200spmm_bsr_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
+        lib.b200spmm_csr16.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, i64, i64, vp,
+                                       i64, C.c_int, vp, C.c_size_t]
+        lib.b200spmm_csr16_workspace_bytes.argtypes = [i64, i64, i64, i64, i64]
+        lib.b200spmm_csr16_workspace_bytes.restype = C.c_size_t
+        lib.b200spmm_csr16_path.argtypes = [i64, vp, i64, i64]
+        lib.b200spmm_csr16_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
         _shim = lib
     return _shim
 

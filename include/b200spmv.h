@@ -261,6 +261,36 @@ B200SPMV_EXPORT int b200spmm_bsr_path(int ab_type, int64_t bs, int a_row_major, 
 B200SPMV_EXPORT void b200spmm_bsr_params(int32_t* k_slab, int32_t* slabs_per_stage, int32_t* stages, int32_t* max_rows_per_cta,
                                          int32_t* chunk_min, int32_t* chunk_factor, int32_t* target_ctas);
 
+/* CSR x dense in half precision (spmm_csr16.cu): C = alpha * A * op(B) + beta * C, A m x k CSR, op(B) k x n and C m x n dense.
+ * Replaces cusparseSpMM for a CSR A with fp16 / bf16 values and fp32 compute.
+ *   ab_type   : type of A's values and of B: 2 = fp16, 14 = bf16 (cudaDataType).
+ *   c_type    : ab_type or 0 = fp32.  alpha / beta (fp32, host or device) and the accumulation are fp32; the epilogue
+ *               alpha * acc + beta * c is fp32 and rounds once to c_type.
+ *   offsets   : m + 1 int32 row offsets, columns: nnz int32 column indices, both with index base `base`.
+ *   B         : op(B)(k, j) = B[k * sbk + j * sbj] (element strides >= 0, as b200spmm_bsr).
+ *   C         : row- or column-major with leading dimension ldc (elements).
+ *   workspace : b200spmm_csr16_workspace_bytes() bytes, 16-byte aligned: the row-major copy of a K-contiguous op(B) (sbk == 1) and
+ *               the carry slots that let a row longer than b200spmm_csr16_params()'s piece be split over several warps.  A NULL,
+ *               misaligned or smaller buffer gathers op(B) in place and walks every row with one warp; both give identical bits.
+ * fp32 FMAs on CUDA cores (no tensor cores: about one flop per gathered byte).  Each C entry is written once in a fixed order (no
+ * atomics: identical bits on every call); beta == 0 never reads C; rows that store nothing get beta * C.  Nothing is read past n,
+ * in ld padding, or in rows of op(B) no stored entry references.  No allocation, no host synchronisation. */
+B200SPMV_EXPORT int b200spmm_csr16(void* stream, int ab_type, int c_type, int64_t m, int64_t k, int64_t n, int64_t nnz,
+                                   const void* offsets, const void* columns, const void* values, int32_t base, const void* alpha,
+                                   const void* beta, int scalars_on_device, const void* B, int64_t sbk, int64_t sbj, void* C, int64_t ldc,
+                                   int c_row_major, void* workspace, size_t workspace_bytes);
+B200SPMV_EXPORT size_t b200spmm_csr16_workspace_bytes(int64_t k, int64_t n, int64_t nnz, int64_t sbk, int64_t sbj);
+/* How b200spmm_csr16 gathers these operands: the 16-bit elements per load, V (2, 4 or 8: one half2 / 64-bit / 128-bit load of a
+ * lane's V columns, V = 1, 2, 4, 8 for n up to 32, 64, 128, more) or 1 (scalar loads: n <= 32, a misaligned view, a leading
+ * dimension that is not a multiple of V, or op(B) not contiguous along n).  With a full workspace a K-contiguous op(B) is read
+ * from its row-major copy: ask with (workspace, n, 1).  0 for bad arguments. */
+B200SPMV_EXPORT int b200spmm_csr16_path(int64_t n, const void* B, int64_t sbk, int64_t sbj);
+/* spmm_csr16's constants: the piece (a row is cut into pieces of at most this many entries at its start + multiples of it; a row
+ * longer than one piece is split when there is a workspace), the entries of a row loaded per coalesced batch, the rows of a
+ * row-tile CTA, warps per CTA, and the most columns of C one lane owns. */
+B200SPMV_EXPORT void b200spmm_csr16_params(int32_t* piece, int32_t* lane_entries, int32_t* tile_rows, int32_t* warps,
+                                           int32_t* max_cols_per_lane);
+
 /* The BLAS-1 part of a CG iteration, fused, all scalars in DEVICE memory (no host synchronisation, CUDA-graph capturable).
  * Replaces the cublasDdot / cublasDaxpy / cublasDnrm2 / cublasDscal calls between two cusparseSpMV calls of gpu_CG
  * (cuSPARSE/cg/cg_example.c:226-286).  fp64; vectors 16-byte aligned; `workspace` = b200cg_workspace_bytes() bytes, zeroed
@@ -388,6 +418,11 @@ B200SPMV_EXPORT int b200spmm_coo_route(const void* matA, const void* matB, const
  * library accepts, no B200SPMV_FORWARD=1, and a class measured at least at parity with the closed library (DESIGN.md 3.17).  A shape
  * mismatch stays native: the call rejects it.  Host logic only. */
 B200SPMV_EXPORT int b200spmm_bsr_route(const void* matA, const void* matB, const void* matC, int opA, int opB, int computeType, int alg);
+/* Where cusparseSpMM_bufferSize / _preprocess / cusparseSpMM send a call with a CSR matA of fp16 / bf16 values: 1 = b200spmm_csr16,
+ * 0 = the closed library.  Native needs opA NON_TRANSPOSE, opB NON_TRANSPOSE or TRANSPOSE, alg DEFAULT or CSR_ALG1 / 2 / 3, int32
+ * indices, B of A's type, C of A's type or fp32, compute type fp32, no strided batch, no B200SPMV_FORWARD=1, and a class measured at
+ * least at parity with the closed library (DESIGN.md 3.18).  A shape mismatch stays native: the call rejects it.  Host logic only. */
+B200SPMV_EXPORT int b200spmm_csr16_route(const void* matA, const void* matB, const void* matC, int opA, int opB, int computeType, int alg);
 /* name of the main kernel the most recent CSR SpMV launched, e.g. "b200::csr_seg_kernel<double>" (bench.py's roofline.kernel) */
 B200SPMV_EXPORT const char* b200spmv_last_csr_kernel(void);
 
