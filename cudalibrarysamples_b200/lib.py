@@ -108,6 +108,12 @@ def shim(build_if_missing: bool = False) -> C.CDLL:
         lib.b200spmm_csr16_workspace_bytes.restype = C.c_size_t
         lib.b200spmm_csr16_path.argtypes = [i64, vp, i64, i64]
         lib.b200spmm_csr16_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
+        lib.b200spmv_csr16.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, vp, vp, C.c_size_t]
+        lib.b200spmv_csr16_workspace_bytes.argtypes = [i64, i64]
+        lib.b200spmv_csr16_workspace_bytes.restype = C.c_size_t
+        lib.b200spmv_csr16_path.argtypes = [vp, vp]
+        lib.b200spmv_csr16_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int]
+        lib.b200spmv_route.argtypes = [C.c_int] * 9 + [i64] * 3
         _shim = lib
     return _shim
 

@@ -115,6 +115,32 @@ B200SPMV_EXPORT int    b200spmv_csr_short_mv_dot(void* stream, int dtype, int64_
                                                  int32_t base, const void* alpha, const void* beta, int scalars_on_device,
                                                  const void* x, void* y, const void* w, double* dot_out, void* workspace);
 
+/* CSR in half precision (spmv_csr16.cu): y = alpha * A * x + beta * y, A rows x cols CSR.  Replaces cusparseSpMV for a CSR A with
+ * fp16 / bf16 values and fp32 compute, opA = NON_TRANSPOSE.  Plan-free: needs no preprocess.
+ *   a_type    : type of A's values and of x: 2 = fp16, 14 = bf16 (cudaDataType).
+ *   y_type    : a_type or 0 = fp32.  alpha / beta (fp32, host or device) and the accumulation are fp32; the epilogue
+ *               alpha * acc + beta * y is fp32 and rounds once to y_type.
+ *   offsets   : rows + 1 int32 row offsets, columns: nnz int32 column indices, both with index base `base`.
+ *   workspace : b200spmv_csr16_workspace_bytes() bytes, 16-byte aligned: two fp32 carry slots per chunk of
+ *               b200spmv_csr16_params()'s chunk entries, so that a row crossing chunks is spread over their warps (split walk).  A
+ *               NULL, misaligned or smaller buffer makes the warp of a row's first chunk add the row's later pieces itself (unsplit
+ *               walk).
+ * Bit-identity: the entries are cut into chunks at fixed positions; the sum of a row's piece inside a chunk depends only on that
+ * piece's products (exact in fp32) and its position in the chunk, and a row adds its pieces in ascending chunk order.  So both walks,
+ * repeated calls and graph replays give identical bits, on any grid or SM count.  Write-once: every y entry and every carry slot is
+ * written exactly once, with no atomics; beta == 0 never reads y; an empty row gets beta * y; nothing past nnz is read, and x only
+ * at stored columns.  No allocation, no host synchronisation (graph-capturable).  Sets b200spmv_last_csr_kernel(). */
+B200SPMV_EXPORT int    b200spmv_csr16(void* stream, int a_type, int y_type, int64_t rows, int64_t cols, int64_t nnz, const void* offsets,
+                                      const void* columns, const void* values, int32_t base, const void* alpha, const void* beta,
+                                      int scalars_on_device, const void* x, void* y, void* workspace, size_t workspace_bytes);
+/* 2 * ceil(nnz / chunk) * 4 bytes; 0 when rows or nnz is 0 */
+B200SPMV_EXPORT size_t b200spmv_csr16_workspace_bytes(int64_t rows, int64_t nnz);
+/* How b200spmv_csr16 streams these arrays: 2 = two entries per lane per load (64-bit columns, 32-bit value pairs: columns 8-byte
+ * and values 4-byte aligned), 1 = scalar loads (a view misaligned by one element).  x and y are always read element by element. */
+B200SPMV_EXPORT int    b200spmv_csr16_path(const void* columns, const void* values);
+/* spmv_csr16's constants: entries per chunk (E), entries per run (a piece adds the sums of the runs it covers), warps per CTA */
+B200SPMV_EXPORT void   b200spmv_csr16_params(int32_t* chunk, int32_t* run, int32_t* warps);
+
 /* CSR, opA = TRANSPOSE (spmv_csr_transpose.cu): y[cols] = alpha * A^T * x[rows] + beta * y; no plan, no workspace; one
  * fp atomic per non-zero, so the summation order (not the tolerance) differs between runs. */
 B200SPMV_EXPORT int    b200spmv_csr_transpose_mv(void* stream, int dtype, int64_t rows, int64_t cols, int64_t nnz,
@@ -380,9 +406,14 @@ B200SPMV_EXPORT int  b200spmv_set_option(const char* key, const char* value);
 B200SPMV_EXPORT void b200spmv_get_stats(uint64_t* native_calls, uint64_t* forwarded_calls, uint64_t* analyze_calls);
 B200SPMV_EXPORT void b200spmv_reset_stats(void);
 /* Which path cusparseSpMV takes for a call of this shape (enum values of cusparse.h / library_types.h passed as int):
- * 0 = handed to the closed library, 1 = the specialised 32-bit-index single-type kernels, 2 = spmv_generic.cu.  Host logic only. */
+ * 0 = handed to the closed library, 1 = the specialised 32-bit-index single-type kernels, 2 = spmv_generic.cu, 3 = b200spmv_csr16
+ * (CSR, int32 indices, A and x fp16 or both bf16, y of A's type or fp32, fp32 compute, opA NON_TRANSPOSE, alg DEFAULT / CSR_ALG1 /
+ * CSR_ALG2, in a class measured at least at parity with the closed library: DESIGN.md 3.19).  Host logic only. */
 B200SPMV_EXPORT int b200spmv_route(int format, int op, int alg, int off_type, int col_type, int a_vtype, int x_vtype, int y_vtype,
                                    int compute_type, int64_t rows, int64_t cols, int64_t nnz);
+/* The same decision over descriptors (cusparseSpMatDescr_t / cusparseDnVecDescr_t passed as void*), as cusparseSpMV_bufferSize /
+ * _preprocess / cusparseSpMV take it: b200spmv_route's codes, 0 under B200SPMV_FORWARD=1 or for NULL descriptors.  Host logic only. */
+B200SPMV_EXPORT int b200spmv_csr16_route(const void* matA, const void* vecX, const void* vecY, int opA, int computeType, int alg);
 /* How many products cusparseSpMM would run on our kernel for these descriptors (cusparseSpMatDescr_t / cusparseDnMatDescr_t passed
  * as void*): 0 = the call goes to the closed library, 1 = an ordinary product, N = a strided batch.  Host logic only. */
 B200SPMV_EXPORT int b200spmm_batch_count(const void* matA, const void* matB, const void* matC);
