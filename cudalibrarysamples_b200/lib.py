@@ -114,6 +114,13 @@ def shim(build_if_missing: bool = False) -> C.CDLL:
         lib.b200spmv_csr16_path.argtypes = [vp, vp]
         lib.b200spmv_csr16_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int]
         lib.b200spmv_route.argtypes = [C.c_int] * 9 + [i64] * 3
+        lib.b200spsm_csr_workspace_bytes.argtypes = [i64, i64, C.c_int]
+        lib.b200spsm_csr_workspace_bytes.restype = C.c_size_t
+        lib.b200spsm_csr_layout.argtypes = [i64, i64, C.c_int, vp]
+        lib.b200spsm_csr_analysis.argtypes = [vp, i64, i64, vp, vp, C.c_int32, C.c_int, C.c_int, C.c_int, vp, vp, vp]
+        lib.b200spsm_csr_solve.argtypes = [vp, C.c_int, i64, i64, C.c_int, vp, vp, vp, C.c_int, i64, vp, i64, i64, vp, i64, i64, vp]
+        lib.b200spsm_csr_tile.argtypes = [i64, C.c_int]
+        lib.b200spsm_route.argtypes = [C.c_int] * 12 + [i64] * 4 + [C.c_int, C.c_int]
         _shim = lib
     return _shim
 

@@ -454,6 +454,55 @@ B200SPMV_EXPORT int b200spmm_bsr_route(const void* matA, const void* matB, const
  * indices, B of A's type, C of A's type or fp32, compute type fp32, no strided batch, no B200SPMV_FORWARD=1, and a class measured at
  * least at parity with the closed library (DESIGN.md 3.18).  A shape mismatch stays native: the call rejects it.  Host logic only. */
 B200SPMV_EXPORT int b200spmm_csr16_route(const void* matA, const void* matB, const void* matC, int opA, int opB, int computeType, int alg);
+/* ---------------------------------------------------------------------------------------------- *
+ * Sparse triangular solve with many right-hand sides (cusparseSpSM; cuSPARSE/spsm_csr):           *
+ *   C = alpha op(T)^-1 op(B), T the selected triangle of the rows x rows CSR matrix A (int32       *
+ *   offsets and columns, index base 0 or 1).  A may store both triangles: entries outside the      *
+ *   selected one are ignored, and with unit = 1 so is the stored diagonal.  lower / unit /         *
+ *   transpose as in b200spsv.h; dtype 0 = fp32, 1 = fp64 (values, B, C, alpha, arithmetic).        *
+ *   return: 0, -1 on invalid arguments (checked before any CUDA call), else the cudaError_t.      *
+ * ---------------------------------------------------------------------------------------------- */
+/* Bytes of the workspace _analysis builds the plan in; pass it to every _solve of that plan (it also holds the solve-state
+ * words, so two solves of one plan must not overlap). */
+B200SPMV_EXPORT size_t b200spsm_csr_workspace_bytes(int64_t rows, int64_t nnz, int transpose);
+/* Byte offsets of the plan's arrays (each 256-byte aligned): SpSV's plan (b200spsv.h: state words, flags, t_off, diag,
+ * t_col, t_vidx) and order[rows], the rows in level order (by level, then by position in the solve direction); the scratch
+ * comes last and the solve reads nothing from it.  offsets[B200SPSM_TOTAL] == b200spsm_csr_workspace_bytes(...).  Returns -1 for
+ * negative sizes. */
+enum { B200SPSM_STATE = 0, B200SPSM_FLAGS, B200SPSM_T_OFF, B200SPSM_DIAG, B200SPSM_T_COL, B200SPSM_T_VIDX, B200SPSM_ORDER, B200SPSM_SCRATCH,
+       B200SPSM_TOTAL, B200SPSM_LAYOUT_N };
+B200SPMV_EXPORT int b200spsm_csr_layout(int64_t rows, int64_t nnz, int transpose, size_t* offsets /* [B200SPSM_LAYOUT_N] */);
+/* Builds the plan and the level order (integer work; values are not read) and clears the state words.  Synchronises the
+ * stream: the levels are computed on the host from the plan read back.  missing_diag (unit = 0: rows without a stored
+ * diagonal) and levels (the number of dependency levels) are written when not NULL. */
+B200SPMV_EXPORT int b200spsm_csr_analysis(void* stream, int64_t rows, int64_t nnz, const void* row_offsets, const void* col_ind,
+                                          int32_t base, int lower, int unit, int transpose, void* workspace, int64_t* missing_diag,
+                                          int64_t* levels);
+/* C = alpha op(T)^-1 op(B) with the plan in workspace, for 0 <= nrhs <= B200SPSM_MAX_NRHS right-hand sides: op(B)(i, j) = B[i * sbi + j * sbk] and
+ * C(i, j) = C[i * sci + j * scj] (any layout, transpose and leading dimension).  values are read now; diag (rows values, or
+ * NULL) replaces the stored diagonal.  alpha is a host pointer, or a device pointer read in the kernel (alpha_on_device = 1).
+ * B may be C.  Two launches, no allocation, no host synchronisation: CUDA-graph capturable.  Each result's bits depend on
+ * the plan and b200spsm_csr_tile(nrhs, scj == 1) only. */
+#define B200SPSM_MAX_NRHS (INT32_MAX - 32)      /* the kernel steps tiles of up to 32 columns in int */
+B200SPMV_EXPORT int b200spsm_csr_solve(void* stream, int dtype, int64_t rows, int64_t nnz, int unit, const void* values, const void* diag,
+                                       const void* alpha, int alpha_on_device, int64_t nrhs, const void* B, int64_t sbi, int64_t sbk,
+                                       void* C, int64_t sci, int64_t scj, void* workspace);
+/* Right-hand sides per tile of the solve kernel: lanes over min(32, nrhs) columns of a C with unit column stride (row-major),
+ * over (entry group, column) with at most 8 columns otherwise (DESIGN.md 3.20).  A power of two.  Pure. */
+B200SPMV_EXPORT int b200spsm_csr_tile(int64_t nrhs, int c_row_major);
+/* Threads per CTA of the solve kernel and the budget (ns of %globaltimer) of any one wait, as b200spsv_csr_params. */
+B200SPMV_EXPORT void b200spsm_csr_params(int32_t* threads_per_cta, uint64_t* spin_budget_ns);
+/* Where cusparseSpSM sends a call of this shape (enum values as int): 0 = the closed library (outside the scope above: not CSR,
+ * 64-bit indices, types other than fp32 / fp64 of one type, CONJUGATE_TRANSPOSE, an alg other than DEFAULT, non-square A,
+ * batch > 1), 1 = within that scope but not in a class measured at least at parity with the closed library (forwarded),
+ * 2 = b200spsm_csr_solve (analysis may still forward a NON_UNIT matrix with a row that stores no diagonal).  No class is
+ * measured native today, so every call in scope answers 1 (DESIGN.md 3.20).  Pure host logic. */
+B200SPMV_EXPORT int b200spsm_route(int format, int opA, int opB, int alg, int off_type, int col_type, int a_vtype, int b_vtype, int c_vtype,
+                                   int compute_type, int fill, int diag, int64_t rows, int64_t cols, int64_t nnz, int64_t nrhs,
+                                   int c_row_major, int batch);
+/* Since the last reset: SpSM solves run natively / SpSM calls handed to the closed library / native analyses. */
+B200SPMV_EXPORT void b200spsm_get_stats(uint64_t* native_calls, uint64_t* forwarded_calls, uint64_t* analysis_calls);
+B200SPMV_EXPORT void b200spsm_reset_stats(void);
 /* name of the main kernel the most recent CSR SpMV launched, e.g. "b200::csr_seg_kernel<double>" (bench.py's roofline.kernel) */
 B200SPMV_EXPORT const char* b200spmv_last_csr_kernel(void);
 
@@ -555,6 +604,19 @@ B200SPMV_EXPORT cusparseStatus_t cusparseSDDMM_preprocess(cusparseHandle_t, cusp
 B200SPMV_EXPORT cusparseStatus_t cusparseSDDMM(cusparseHandle_t, cusparseOperation_t, cusparseOperation_t, const void*,
                                                cusparseConstDnMatDescr_t, cusparseConstDnMatDescr_t, const void*,
                                                cusparseSpMatDescr_t, cudaDataType, cusparseSDDMMAlg_t, void*);
+/* cusparse.h:5794-5842 -- spsm_csr_example.c */
+B200SPMV_EXPORT cusparseStatus_t cusparseSpSM_createDescr(cusparseSpSMDescr_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseSpSM_destroyDescr(cusparseSpSMDescr_t);
+B200SPMV_EXPORT cusparseStatus_t cusparseSpSM_bufferSize(cusparseHandle_t, cusparseOperation_t, cusparseOperation_t, const void*,
+                                                         cusparseConstSpMatDescr_t, cusparseConstDnMatDescr_t, cusparseDnMatDescr_t,
+                                                         cudaDataType, cusparseSpSMAlg_t, cusparseSpSMDescr_t, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseSpSM_analysis(cusparseHandle_t, cusparseOperation_t, cusparseOperation_t, const void*,
+                                                       cusparseConstSpMatDescr_t, cusparseConstDnMatDescr_t, cusparseDnMatDescr_t,
+                                                       cudaDataType, cusparseSpSMAlg_t, cusparseSpSMDescr_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseSpSM_solve(cusparseHandle_t, cusparseOperation_t, cusparseOperation_t, const void*,
+                                                    cusparseConstSpMatDescr_t, cusparseConstDnMatDescr_t, cusparseDnMatDescr_t,
+                                                    cudaDataType, cusparseSpSMAlg_t, cusparseSpSMDescr_t);
+B200SPMV_EXPORT cusparseStatus_t cusparseSpSM_updateMatrix(cusparseHandle_t, cusparseSpSMDescr_t, void*, cusparseSpSMUpdate_t);
 #ifdef __cplusplus
 }
 #endif
