@@ -35,8 +35,8 @@ namespace b200 {
 #ifndef B200_FLAT_MIN_CTAS
 #define B200_FLAT_MIN_CTAS 10     // x 128 threads, 48 registers (swept on an earlier GPU, not re-swept on the H100: scripts/sweep.py FLAT)
 #endif
-#ifndef B200_FLAT_BATCH        // steps whose col / val loads are all issued before the first gather -- fp64; the fp32 kernel has the
-#define B200_FLAT_BATCH 4      // registers for all 8 steps of a chunk (swept on an earlier GPU, not re-swept on the H100: scripts/sweep.py FLAT)
+#ifndef B200_FLAT_BATCH        // steps whose col / val loads are all issued before the first gather, fp64 and (unless
+#define B200_FLAT_BATCH 4      // B200_FLAT_BATCH32 says otherwise) fp32; swept with the resident CTAs on the H100, DESIGN.md §3.2
 #endif
 #ifndef B200_FLAT_STEPS
 #define B200_FLAT_STEPS 8
@@ -65,9 +65,13 @@ constexpr int FLAT_BATCH64 = B200_FLAT_BATCH;
 #ifdef B200_FLAT_BATCH32
 constexpr int FLAT_BATCH32 = B200_FLAT_BATCH32;
 #else
-constexpr int FLAT_BATCH32 = (2 * B200_FLAT_BATCH <= B200_FLAT_STEPS) ? 2 * B200_FLAT_BATCH : B200_FLAT_BATCH;
+constexpr int FLAT_BATCH32 = B200_FLAT_BATCH;      // fp32 too: a batch of 4 ran fp32 R-MAT 1 M 6 % faster than 8 on the H100 (DESIGN.md §3.2)
 #endif
 constexpr int SCAN_ITEMS = 2048;                   // items per block of the preprocessing scans
+#ifndef B200_FLAT_FIXUP_AHEAD
+#define B200_FLAT_FIXUP_AHEAD 8                    // CTA partials csr_flat_fixup_kernel loads per round trip
+#endif
+constexpr int FIXUP_AHEAD = B200_FLAT_FIXUP_AHEAD;
 static_assert(FLAT_STEPS % FLAT_BATCH64 == 0 && FLAT_STEPS % FLAT_BATCH32 == 0, "steps per chunk must be a multiple of the batch");
 
 // Hot columns of x.  Preprocess picks the most-used columns whose values fit B200_FLAT_HOT_BYTES, and every SpMV first packs
@@ -516,9 +520,27 @@ __global__ void __launch_bounds__(256) csr_flat_fixup_kernel(const FlatArgs<T> a
     const bool starts_row = t == 0 || (__ldg(a.plan.endmask + t * FLAT_CTA_WORDS - 1) >> 31);
     if (!has && !starts_row) return;                       // CTA t lies inside a row that started earlier
     double sum = has ? __ldcg(a.plan.cta_last + t) : __ldcg(a.plan.cta_first + t);
+    // Add cta_first of the CTAs the row runs through, up to the one it ends in (cta_flags != 0), in CTA order.  The heaviest
+    // rows of a skewed matrix cross dozens of CTAs: FIXUP_AHEAD CTAs are loaded per L2 round trip instead of one after the
+    // other.  The last CTA always ends a row, so clamping the look-ahead to it changes no sum.
     long long u = t + 1;
-    while (__ldcg(a.plan.cta_flags + u) == 0) { sum += __ldcg(a.plan.cta_first + u); u++; }
-    sum += __ldcg(a.plan.cta_first + u);
+    for (bool done = false; !done; ) {
+        int    fl[FIXUP_AHEAD];
+        double fs[FIXUP_AHEAD];
+#pragma unroll
+        for (int k = 0; k < FIXUP_AHEAD; k++) {
+            const long long v = min(u + k, nctas - 1);
+            fl[k] = __ldcg(a.plan.cta_flags + v);
+            fs[k] = __ldcg(a.plan.cta_first + v);
+        }
+#pragma unroll
+        for (int k = 0; k < FIXUP_AHEAD; k++) {
+            if (done) continue;
+            sum += fs[k];
+            if (fl[k] != 0) { done = true; u += k; }
+        }
+        if (!done) u += FIXUP_AHEAD;
+    }
     const int row = __ldg(a.plan.nzrow + __ldg(a.plan.chunk_run + u * (FLAT_CTA_NNZ / PLAN_CHUNK)) + 1);
     flat_store_y(a.y + row, alpha, (T)sum, beta);
 }
