@@ -55,6 +55,12 @@ static int apply(Config& c, const char* key, const char* value) {
         else return -1;
         return 0;
     }
+    if (!strcmp(key, "B200SPMV_ZCSR")) {
+        if (!value || !value[0] || !strcmp(value, "auto")) c.zcsr = 0;
+        else if (!strcmp(value, "on")) c.zcsr = 1;
+        else return -1;
+        return 0;
+    }
     return -1;
 }
 
@@ -63,7 +69,8 @@ Config& config() {
     static std::once_flag once;
     std::call_once(once, [] {
         static const char* keys[] = {"B200SPMV_CSR_KERNEL", "B200SPMV_COO_KERNEL", "B200SPMV_TILE_ORDER", "B200SPMV_PDL",
-                                     "B200SPMV_SEG_DENSE", "B200SPMV_SELL_GENERIC", "B200SPMV_FLAT", "B200SPMV_FLAT_QUIET", "B200SPMV_SHORT", "B200SPMV_GENERIC"};
+                                     "B200SPMV_SEG_DENSE", "B200SPMV_SELL_GENERIC", "B200SPMV_FLAT", "B200SPMV_FLAT_QUIET", "B200SPMV_SHORT", "B200SPMV_GENERIC",
+                                     "B200SPMV_ZCSR"};
         for (const char* k : keys)
             if (const char* v = getenv(k)) apply(c, k, v);
     });

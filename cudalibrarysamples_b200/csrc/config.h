@@ -20,6 +20,9 @@ struct Config {
                             //   all: also COO and Sliced-ELL of those kinds, Sliced-ELL transposes, strided-batch SpMM -- written
                             //        and emulated on the CPU, their first hardware run is tests/test_zz_unverified_gpu.py;
                             //   off: everything of that kind goes to the closed library
+    int zcsr        = 0;    // B200SPMV_ZCSR = auto|on: cusparseSpMV on a double-complex CSR A.  auto (0, default): b200spmv_csr_z
+                            //   only in the classes measured at least at parity (none today, DESIGN.md 3.21); on (1): every call
+                            //   in b200spmv_csr_z's class
 };
 
 Config& config();

@@ -114,6 +114,10 @@ def shim(build_if_missing: bool = False) -> C.CDLL:
         lib.b200spmv_csr16_path.argtypes = [vp, vp]
         lib.b200spmv_csr16_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int]
         lib.b200spmv_route.argtypes = [C.c_int] * 9 + [i64] * 3
+        lib.b200spmv_csr_z.argtypes = [vp, C.c_int, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, vp, vp, C.c_size_t]
+        lib.b200spmv_csr_z_workspace_bytes.argtypes = [i64, i64]
+        lib.b200spmv_csr_z_workspace_bytes.restype = C.c_size_t
+        lib.b200spmv_csr_z_params.argtypes = [vp, vp, vp]
         lib.b200spsm_csr_workspace_bytes.argtypes = [i64, i64, C.c_int]
         lib.b200spsm_csr_workspace_bytes.restype = C.c_size_t
         lib.b200spsm_csr_layout.argtypes = [i64, i64, C.c_int, vp]

@@ -141,6 +141,32 @@ B200SPMV_EXPORT int    b200spmv_csr16_path(const void* columns, const void* valu
 /* spmv_csr16's constants: entries per chunk (E), entries per run (a piece adds the sums of the runs it covers), warps per CTA */
 B200SPMV_EXPORT void   b200spmv_csr16_params(int32_t* chunk, int32_t* run, int32_t* warps);
 
+/* CSR in double complex (spmv_csr_z.cu): y = alpha * op(A) * x + beta * y, A rows x cols CSR.  Replaces cusparseSpMV for a CSR A
+ * with CUDA_C_64F values, x, y and compute.
+ *   op        : 0 = NON_TRANSPOSE (x has cols entries, y rows), 1 = TRANSPOSE, 2 = CONJUGATE_TRANSPOSE (x has rows entries, y cols).
+ *   offsets   : rows + 1 int32 row offsets, columns: nnz int32 column indices, both with index base `base`.
+ *   values, x, y : cuDoubleComplex, 16-byte aligned (any cuDoubleComplex array is; a misaligned y, or values / x when nnz > 0, is
+ *               rejected with -1).
+ *   alpha, beta : cuDoubleComplex, on the host or (scalars_on_device) on the device.
+ *   workspace : op = 0 only: b200spmv_csr_z_workspace_bytes() bytes, 16-byte aligned: two cuDoubleComplex carry slots per chunk of
+ *               b200spmv_csr_z_params()'s chunk entries (split walk).  A NULL, misaligned or smaller buffer gives the unsplit walk, with
+ *               the same bits.  op = 1 / 2 use none.
+ * Arithmetic (fixed with correctly rounded intrinsics, no contraction): a product is (fma(ar, br, -(ai * bi)), fma(ar, bi, ai * br));
+ * the epilogue is (fma(al_r, acc_r, fma(-al_i, acc_i, t_r)), fma(al_r, acc_i, fma(al_i, acc_r, t_i))) with t = beta * y as a
+ * product, t = 0 when beta == 0.
+ * op = 0 is deterministic as b200spmv_csr16 is: chunks at fixed positions, each piece of a row summed in a fixed order, pieces in
+ * ascending chunk order; both walks, repeated calls and graph replays give identical bits, no atomics; beta == 0 never reads y and an
+ * empty row gets beta * y.  op = 1 / 2 scale y by beta, then add alpha * (v * x[r]) (conj(v) for op = 2) into y[c] with two fp64
+ * atomic adds per entry: the order of the additions is not fixed.  No allocation, no host synchronisation (graph-capturable).  Sets
+ * b200spmv_last_csr_kernel().  Returns 0, -1 for a rejected argument, or a cudaError_t. */
+B200SPMV_EXPORT int    b200spmv_csr_z(void* stream, int op, int64_t rows, int64_t cols, int64_t nnz, const void* offsets, const void* columns,
+                                      const void* values, int32_t base, const void* alpha, const void* beta, int scalars_on_device,
+                                      const void* x, void* y, void* workspace, size_t workspace_bytes);
+/* 2 * ceil(nnz / chunk) * 16 bytes; 0 when rows or nnz is 0 */
+B200SPMV_EXPORT size_t b200spmv_csr_z_workspace_bytes(int64_t rows, int64_t nnz);
+/* spmv_csr_z's constants: entries per chunk (E), entries per run (a piece adds the sums of the runs it covers), warps per CTA */
+B200SPMV_EXPORT void   b200spmv_csr_z_params(int32_t* chunk, int32_t* run, int32_t* warps);
+
 /* CSR, opA = TRANSPOSE (spmv_csr_transpose.cu): y[cols] = alpha * A^T * x[rows] + beta * y; no plan, no workspace; one
  * fp atomic per non-zero, so the summation order (not the tolerance) differs between runs. */
 B200SPMV_EXPORT int    b200spmv_csr_transpose_mv(void* stream, int dtype, int64_t rows, int64_t cols, int64_t nnz,
@@ -398,6 +424,8 @@ B200SPMV_EXPORT int b200spmv_sell_generic_mv(void* stream, int off64, int col64,
  *   B200SPMV_SHORT = auto|on|off
  *   B200SPMV_GENERIC = off|csr|all (what spmv_generic.cu serves instead of the closed library: nothing / CSR [default] / also
  *                      COO, Sliced-ELL and strided-batch SpMM, which have not had their first hardware run yet)
+ *   B200SPMV_ZCSR = auto|on (cusparseSpMV on a double-complex CSR A: auto [default] = b200spmv_csr_z only in the classes measured at
+ *                      least at parity with the closed library (none today, DESIGN.md 3.21); on = every call in its class)
  * returns 0, or -1 for an unknown key / value. */
 B200SPMV_EXPORT int  b200spmv_set_option(const char* key, const char* value);
 /* Call counters of the cuSPARSE-symbol layer: SpMV calls that ran on our kernels, SpMV calls handed to the closed library
@@ -408,11 +436,14 @@ B200SPMV_EXPORT void b200spmv_reset_stats(void);
 /* Which path cusparseSpMV takes for a call of this shape (enum values of cusparse.h / library_types.h passed as int):
  * 0 = handed to the closed library, 1 = the specialised 32-bit-index single-type kernels, 2 = spmv_generic.cu, 3 = b200spmv_csr16
  * (CSR, int32 indices, A and x fp16 or both bf16, y of A's type or fp32, fp32 compute, opA NON_TRANSPOSE, alg DEFAULT / CSR_ALG1 /
- * CSR_ALG2, in a class measured at least at parity with the closed library: DESIGN.md 3.19).  Host logic only. */
+ * CSR_ALG2, in a class measured at least at parity with the closed library: DESIGN.md 3.19), 4 = b200spmv_csr_z (CSR, int32
+ * indices, A, x, y and compute CUDA_C_64F, alg DEFAULT / CSR_ALG1 / CSR_ALG2, in a class measured at least at parity with the closed
+ * library: DESIGN.md 3.21).  Host logic only. */
 B200SPMV_EXPORT int b200spmv_route(int format, int op, int alg, int off_type, int col_type, int a_vtype, int x_vtype, int y_vtype,
                                    int compute_type, int64_t rows, int64_t cols, int64_t nnz);
 /* The same decision over descriptors (cusparseSpMatDescr_t / cusparseDnVecDescr_t passed as void*), as cusparseSpMV_bufferSize /
- * _preprocess / cusparseSpMV take it: b200spmv_route's codes, 0 under B200SPMV_FORWARD=1 or for NULL descriptors.  Host logic only. */
+ * _preprocess / cusparseSpMV take it: b200spmv_route's codes, 0 under B200SPMV_FORWARD=1 or for NULL descriptors, for descriptors of
+ * any value type (complex ones included).  Host logic only. */
 B200SPMV_EXPORT int b200spmv_csr16_route(const void* matA, const void* vecX, const void* vecY, int opA, int computeType, int alg);
 /* How many products cusparseSpMM would run on our kernel for these descriptors (cusparseSpMatDescr_t / cusparseDnMatDescr_t passed
  * as void*): 0 = the call goes to the closed library, 1 = an ordinary product, N = a strided batch.  Host logic only. */
