@@ -108,6 +108,15 @@ def shim(build_if_missing: bool = False) -> C.CDLL:
         lib.b200spmm_csr16_workspace_bytes.restype = C.c_size_t
         lib.b200spmm_csr16_path.argtypes = [i64, vp, i64, i64]
         lib.b200spmm_csr16_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
+        lib.b200spmm_csr_t.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, i64, i64, vp,
+                                       i64, C.c_int, C.c_int, vp, C.c_size_t]
+        lib.b200spmm_csr_t_plan.argtypes = [vp, i64, i64, i64, vp, vp, C.c_int32, vp, C.c_size_t]
+        lib.b200spmm_csr_t_layout.argtypes = [C.c_int, i64, i64, i64, i64, i64, i64, vp]
+        lib.b200spmm_csr_t_layout.restype = C.c_size_t
+        lib.b200spmm_csr_t_workspace_bytes.argtypes = [C.c_int, i64, i64, i64, i64, i64, i64]
+        lib.b200spmm_csr_t_workspace_bytes.restype = C.c_size_t
+        lib.b200spmm_csr_t_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]
+        lib.b200spmv_plan_trusted.argtypes = [vp, vp, C.c_int]
         lib.b200spmv_csr16.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, vp, vp, C.c_size_t]
         lib.b200spmv_csr16_workspace_bytes.argtypes = [i64, i64]
         lib.b200spmv_csr16_workspace_bytes.restype = C.c_size_t

@@ -343,6 +343,37 @@ B200SPMV_EXPORT int b200spmm_csr16_path(int64_t n, const void* B, int64_t sbk, i
 B200SPMV_EXPORT void b200spmm_csr16_params(int32_t* piece, int32_t* lane_entries, int32_t* tile_rows, int32_t* warps,
                                            int32_t* max_cols_per_lane);
 
+/* Transposed CSR x dense (spmm_csr_t.cu): C = alpha * op(A) * op(B) + beta * C with op(A) = A^T (= A^H: the types are real), A rows x
+ * cols CSR with int32 offsets / columns (base 0 or 1), op(B) rows x n, C cols x n.  Replaces cusparseSpMM for a CSR A with opA =
+ * TRANSPOSE / CONJUGATE_TRANSPOSE.  No atomics: a transposed plan (the CSC form of A's pattern) is built in the workspace, values are
+ * gathered into it on every call, and the opA = N kernels run on A^T as a cols x rows CSR matrix (b200spmm_csr_ws for fp32 / fp64,
+ * b200spmm_csr16 for fp16 / bf16).  The result is bit-identical to that opA = N call on the explicit transpose: deterministic.
+ *   dtype / c_type : cudaDataType of A and B / of C: 0 / 0 (fp32), 1 / 1 (fp64), 2 or 14 / the same or 0 (fp16 or bf16, fp32 compute,
+ *                    fp32 host or device scalars).
+ *   B              : op(B)(k, j) = B[k * sbk + j * sbj].  fp32 / fp64 take op(B) row-major (sbj == 1) or column-major (sbk == 1).
+ *   plan_valid     : nonzero when the workspace already holds the plan of this pattern (b200spmm_csr_t_plan or an earlier call with
+ *                    the same offsets and columns), so only the values are gathered; 0 rebuilds the plan first.
+ *   workspace      : b200spmm_csr_t_workspace_bytes() bytes, 16-byte aligned.
+ * Returns -1 with nothing launched on a bad argument: unknown or mismatched types, a NULL, misaligned or short workspace, sizes past
+ * the limits of the opA = N entry point, an fp32 / fp64 op(B) that is neither row- nor column-major.  No allocation, no host
+ * synchronisation: graph-capturable. */
+B200SPMV_EXPORT int b200spmm_csr_t(void* stream, int dtype, int c_type, int64_t rows, int64_t cols, int64_t n, int64_t nnz,
+                                   const void* offsets, const void* columns, const void* values, int32_t base, const void* alpha,
+                                   const void* beta, int scalars_on_device, const void* B, int64_t sbk, int64_t sbj, void* C, int64_t ldc,
+                                   int c_row_major, int plan_valid, void* workspace, size_t workspace_bytes);
+/* Builds the transposed plan of A's pattern in the workspace (at least offsets[4] of b200spmm_csr_t_layout bytes: the plan and the
+ * sort scratch).  -1 on bad arguments, nothing launched. */
+B200SPMV_EXPORT int b200spmm_csr_t_plan(void* stream, int64_t rows, int64_t cols, int64_t nnz, const void* offsets, const void* columns,
+                                        int32_t base, void* workspace, size_t workspace_bytes);
+/* The workspace of b200spmm_csr_t: total bytes (0 on bad arguments).  offsets (6 entries, or NULL) receives the byte offsets of
+ * tOff (cols + 1 int32 CSC column pointers, base 0), tRow (nnz int32 rows, base 0, ascending within a column), perm (nnz int32 CSR
+ * positions), the sort scratch, tVal (nnz values of A's type) and the opA = N kernel's own workspace.  Every part is 256-byte aligned;
+ * the plan and the scratch depend on (cols, nnz) only. */
+B200SPMV_EXPORT size_t b200spmm_csr_t_layout(int dtype, int64_t rows, int64_t cols, int64_t n, int64_t nnz, int64_t sbk, int64_t sbj,
+                                             size_t* offsets);
+B200SPMV_EXPORT size_t b200spmm_csr_t_workspace_bytes(int dtype, int64_t rows, int64_t cols, int64_t n, int64_t nnz, int64_t sbk,
+                                                      int64_t sbj);
+
 /* The BLAS-1 part of a CG iteration, fused, all scalars in DEVICE memory (no host synchronisation, CUDA-graph capturable).
  * Replaces the cublasDdot / cublasDaxpy / cublasDnrm2 / cublasDscal calls between two cusparseSpMV calls of gpu_CG
  * (cuSPARSE/cg/cg_example.c:226-286).  fp64; vectors 16-byte aligned; `workspace` = b200cg_workspace_bytes() bytes, zeroed
@@ -485,6 +516,18 @@ B200SPMV_EXPORT int b200spmm_bsr_route(const void* matA, const void* matB, const
  * indices, B of A's type, C of A's type or fp32, compute type fp32, no strided batch, no B200SPMV_FORWARD=1, and a class measured at
  * least at parity with the closed library (DESIGN.md 3.18).  A shape mismatch stays native: the call rejects it.  Host logic only. */
 B200SPMV_EXPORT int b200spmm_csr16_route(const void* matA, const void* matB, const void* matC, int opA, int opB, int computeType, int alg);
+/* Where cusparseSpMM sends a call with a CSR matA and opA TRANSPOSE / CONJUGATE_TRANSPOSE, given the call's externalBuffer: 1 =
+ * b200spmm_csr_t, 0 = the closed library.  Native needs opA TRANSPOSE (the closed library refuses CONJUGATE_TRANSPOSE for these real
+ * types: such calls keep its verdict), alg DEFAULT or CSR_ALG1, int32 indices, no strided batch, a non-NULL buffer,
+ * no B200SPMV_FORWARD=1, opB NON_TRANSPOSE (opB = T was not measured); fp32 / fp64 with A, B, C and compute of one type, or fp16 /
+ * bf16 with B of A's type, C of A's type or fp32 and compute fp32; and a class measured at least at parity with the closed library
+ * (DESIGN.md 3.22).  Host logic only. */
+B200SPMV_EXPORT int b200spmm_csr_t_route(const void* matA, const void* matB, const void* matC, int opA, int opB, int computeType, int alg,
+                                         void* buffer);
+/* Whether the shim trusts `buffer` to hold matA's plan of a kind: 0 = the CSR SpMV plan (cusparseSpMV_preprocess), 1 = the
+ * transposed SpMM plan (cusparseSpMM_preprocess).  A buffer holds the plan of its latest preprocess only, and each kind trusts only
+ * its own; cusparseCsrSetPointers, a new bufferSize query of that operation and cusparseDestroySpMat drop the trust.  Host logic only. */
+B200SPMV_EXPORT int b200spmv_plan_trusted(const void* matA, void* buffer, int kind);
 /* ---------------------------------------------------------------------------------------------- *
  * Sparse triangular solve with many right-hand sides (cusparseSpSM; cuSPARSE/spsm_csr):           *
  *   C = alpha op(T)^-1 op(B), T the selected triangle of the rows x rows CSR matrix A (int32       *
