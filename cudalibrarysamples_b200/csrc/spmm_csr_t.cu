@@ -12,9 +12,9 @@
 //   tRow[nnz]       the row of each CSC entry (base 0);
 //   perm[nnz]       the CSR position of each CSC entry.
 // Within a column, entries are in ascending row order (that of scipy.sparse.csr_matrix.tocsc()), so the plan is a pure function of
-// the pattern.  It is a stable LSD radix sort of the entry indices by column, 8 bits per pass (as many passes as cols - 1 needs
-// bits, at least one): per tile of RT_TILE entries a digit histogram, a scan of the histograms per digit, then a scatter that ranks
-// the entries of a tile in their CSR order.  Stable ranking keeps equal columns in entry order, and entry order is row order.  The
+// the pattern.  It is a stable LSD radix sort of the entry indices by column (radix_sort.cuh, shared with convert.cu), 8 bits per
+// pass (as many passes as cols - 1 needs bits, at least one): per tile of RT_TILE entries a digit histogram, a scan of the histograms
+// per digit, then a scatter that ranks the entries of a tile in their CSR order.  Stable ranking keeps equal columns in entry order, and entry order is row order.  The
 // sorted keys give tOff, a binary search over the row offsets gives tRow.  Each call then gathers tVal[k] = val[perm[k]], so new
 // values (cusparseSpMatSetValues) need no new plan; a new pattern does.
 //
@@ -22,6 +22,7 @@
 //   [ plan: tOff | tRow | perm ][ sort scratch: keys x2 | indices x2 | histograms | digit totals ][ tVal ][ the N kernel's workspace ]
 // The plan and the scratch depend on (cols, nnz) only.  No allocation, no host synchronisation: graph-capturable.
 #include "spmv_common.cuh"
+#include "radix_sort.cuh"
 #include "../../include/b200spmv.h"
 
 #include <algorithm>
@@ -29,20 +30,19 @@
 
 namespace b200 {
 
-constexpr int RT_THREADS = 256;                    // threads of every plan kernel
-constexpr int RT_ITEMS = 8;                        // entries per thread per pass: one round of RT_THREADS entries each
-constexpr int RT_TILE = RT_THREADS * RT_ITEMS;     // entries per tile
-constexpr int RT_BITS = 8, RT_BINS = 1 << RT_BITS;
 constexpr int RT_WARPS = RT_THREADS / 32;
 constexpr int T_F32 = 0, T_F64 = 1, T_F16 = 2, T_BF16 = 14;   // cudaDataType values
 
 static_assert(RT_BINS == RT_THREADS, "one thread per digit");
 
-// key of entry i: its column (base removed)
-__device__ __forceinline__ int rt_key(const int* keys, int sub, int i) { return __ldg(keys + i) - sub; }
+// key of entry i: keys[i], or keys[kidx[i]] when the keys are read through an earlier permutation, less sub (a base)
+__device__ __forceinline__ int rt_key(const int* keys, int sub, const int* kidx, int i) {
+    return __ldg(keys + (kidx ? __ldg(kidx + i) : i)) - sub;
+}
 
 // hist[d * ntiles + t] = entries of tile t whose digit is d
-__global__ void __launch_bounds__(RT_THREADS) spmm_csr_t_hist_kernel(const int* keys, int sub, int nnz, int shift, int* hist, int ntiles) {
+__global__ void __launch_bounds__(RT_THREADS) spmm_csr_t_hist_kernel(const int* keys, int sub, const int* kidx, int nnz, int shift,
+                                                                  int* hist, int ntiles) {
     __shared__ int h[RT_BINS];
     h[threadIdx.x] = 0;
     __syncthreads();
@@ -50,7 +50,7 @@ __global__ void __launch_bounds__(RT_THREADS) spmm_csr_t_hist_kernel(const int* 
 #pragma unroll
     for (int r = 0; r < RT_ITEMS; r++) {
         const int i = t0 + r * RT_THREADS + (int)threadIdx.x;
-        if (i < nnz) atomicAdd(&h[(rt_key(keys, sub, i) >> shift) & (RT_BINS - 1)], 1);
+        if (i < nnz) atomicAdd(&h[(rt_key(keys, sub, kidx, i) >> shift) & (RT_BINS - 1)], 1);
     }
     __syncthreads();
     hist[(long long)threadIdx.x * ntiles + blockIdx.x] = h[threadIdx.x];
@@ -77,9 +77,9 @@ __global__ void __launch_bounds__(RT_THREADS) spmm_csr_t_scan_kernel(int* hist, 
 // Stable scatter of one tile: entry i goes to (entries of smaller digits) + (entries of its digit in earlier tiles) + (entries of its
 // digit before it in this tile).  Within a round of RT_THREADS entries, warps in order and lanes in order; rounds in order.
 // vals == nullptr: the indices are the entry positions themselves (the first pass).
-__global__ void __launch_bounds__(RT_THREADS) spmm_csr_t_scatter_kernel(const int* keys, int sub, const int* vals, int nnz, int shift,
-                                                                     const int* hist, const int* tot, int ntiles, int* keys_out,
-                                                                     int* vals_out) {
+__global__ void __launch_bounds__(RT_THREADS) spmm_csr_t_scatter_kernel(const int* keys, int sub, const int* kidx, const int* vals, int nnz,
+                                                                     int shift, const int* hist, const int* tot, int ntiles,
+                                                                     int* keys_out, int* vals_out) {
     using Scan = cub::BlockScan<int, RT_THREADS>;
     __shared__ typename Scan::TempStorage tmp;
     __shared__ int base[RT_BINS];                      // next position of each digit
@@ -97,7 +97,7 @@ __global__ void __launch_bounds__(RT_THREADS) spmm_csr_t_scatter_kernel(const in
     for (int r = 0; r < RT_ITEMS; r++) {
         const int i = t0 + r * RT_THREADS + tid;
         const bool live = i < nnz;
-        const int key = live ? rt_key(keys, sub, i) : 0;
+        const int key = live ? rt_key(keys, sub, kidx, i) : 0;
         const int d = live ? (key >> shift) & (RT_BINS - 1) : -1;
         const unsigned peers = __match_any_sync(0xffffffffu, d);
         const int rank = __popc(peers & lt);
@@ -120,26 +120,29 @@ __global__ void __launch_bounds__(RT_THREADS) spmm_csr_t_scatter_kernel(const in
     }
 }
 
-// tOff from the sorted columns: entry k is the first of every column in (key[k - 1], key[k]]; k = nnz closes the columns up to cols.
-__global__ void __launch_bounds__(RT_THREADS) spmm_csr_t_offsets_kernel(const int* sorted, int nnz, int cols, int* t_off) {
+// Offsets from sorted keys (less sub): entry k is the first of every key in (key[k - 1], key[k]]; k = nnz closes the keys up to
+// nkeys.  Clamped to [0, nkeys]: keys from a caller's array may hold anything.
+__global__ void __launch_bounds__(RT_THREADS) spmm_csr_t_offsets_kernel(const int* sorted, int sub, int nnz, int nkeys, int base,
+                                                                     int* t_off) {
     for (long long k = (long long)blockIdx.x * RT_THREADS + threadIdx.x; k <= nnz; k += (long long)gridDim.x * RT_THREADS) {
-        const int prev = k > 0 ? sorted[k - 1] : -1, cur = k < nnz ? sorted[k] : cols;
-        for (int c = prev + 1; c <= cur; c++) t_off[c] = (int)k;
+        const long long prev = k > 0 ? (long long)sorted[k - 1] - sub : -1, cur = k < nnz ? (long long)sorted[k] - sub : nkeys;
+        const long long hi = cur < nkeys ? cur : nkeys;
+        for (long long c = prev + 1 > 0 ? prev + 1 : 0; c <= hi; c++) t_off[c] = (int)k + base;
     }
 }
 
-// tRow[k] = the row holding CSR entry perm[k]: the last r with off[r] - base <= perm[k]
+// tRow[k] = out_base + the row holding CSR entry perm[k] (entry k when perm is NULL): the last r with off[r] - base <= perm[k]
 __global__ void __launch_bounds__(RT_THREADS) spmm_csr_t_rows_kernel(const int* off, int base, int rows, const int* perm, int nnz,
-                                                                  int* t_row) {
+                                                                  int out_base, int* t_row) {
     const int k = (int)blockIdx.x * RT_THREADS + (int)threadIdx.x;
     if (k >= nnz) return;
-    const int x = perm[k];
+    const int x = perm ? perm[k] : k;
     int lo = 0, hi = rows;
     while (hi - lo > 1) {
         const int mid = (lo + hi) >> 1;
         if (__ldg(off + mid) - base <= x) lo = mid; else hi = mid;
     }
-    t_row[k] = lo;
+    t_row[k] = lo + out_base;
 }
 
 // tVal[k] = val[perm[k]], bit for bit (W: the value's width as an unsigned type)
@@ -152,31 +155,83 @@ __global__ void __launch_bounds__(RT_THREADS) spmm_csr_t_gather_kernel(const W* 
 // ------------------------------------------------------------------------------------------------ host side
 static size_t up256(size_t b) { return (b + 255) / 256 * 256; }
 static int64_t rt_ntiles(int64_t nnz) { return (nnz + RT_TILE - 1) / RT_TILE; }
-static int rt_passes(int64_t cols) {
+static unsigned rt_grid(int64_t n) { return (unsigned)((n + RT_THREADS - 1) / RT_THREADS); }
+
+int rt_passes(int64_t nkeys) {
     int bits = 0;
-    while (bits < 32 && ((int64_t)1 << bits) < cols) bits++;   // bits of cols - 1
+    while (bits < 32 && ((int64_t)1 << bits) < nkeys) bits++;   // bits of nkeys - 1
     return bits == 0 ? 1 : (bits + RT_BITS - 1) / RT_BITS;
 }
+
+size_t rt_scratch_bytes(int64_t n) {
+    return 4 * up256((size_t)n * 4) + up256((size_t)RT_BINS * rt_ntiles(n) * 4) + up256((size_t)RT_BINS * 4);
+}
+
+RtScratch rt_scratch(char* base, int64_t n) {
+    const size_t e = up256((size_t)n * 4);
+    RtScratch s;
+    s.k[0] = (int*)base;
+    s.k[1] = (int*)(base + e);
+    s.v[0] = (int*)(base + 2 * e);
+    s.v[1] = (int*)(base + 3 * e);
+    s.hist = (int*)(base + 4 * e);
+    s.tot = (int*)(base + 4 * e + up256((size_t)RT_BINS * rt_ntiles(n) * 4));
+    return s;
+}
+
+void rt_sort(cudaStream_t st, const int* keys, int sub, const int* kidx, const int* vals, int n, int64_t nkeys, const RtScratch& s,
+             int* vals_out, const int** sorted_keys, const int** sorted_vals) {
+    const int ntiles = (int)rt_ntiles(n), passes = rt_passes(nkeys);
+    for (int p = 0; p < passes; p++) {
+        const int shift = p * RT_BITS;
+        int* ko = s.k[p & 1];
+        int* vo = p == passes - 1 && vals_out ? vals_out : s.v[p & 1];
+        spmm_csr_t_hist_kernel<<<ntiles, RT_THREADS, 0, st>>>(keys, sub, kidx, n, shift, s.hist, ntiles);
+        spmm_csr_t_scan_kernel<<<RT_BINS, RT_THREADS, 0, st>>>(s.hist, ntiles, s.tot);
+        spmm_csr_t_scatter_kernel<<<ntiles, RT_THREADS, 0, st>>>(keys, sub, kidx, vals, n, shift, s.hist, s.tot, ntiles, ko, vo);
+        keys = ko; vals = vo; kidx = nullptr; sub = 0;
+    }
+    if (sorted_keys) *sorted_keys = keys;
+    if (sorted_vals) *sorted_vals = vals;
+}
+
+void rt_offsets(cudaStream_t st, const int* keys, int sub, int n, int64_t nkeys, int base, int* out) {
+    const unsigned grid = (unsigned)std::min<long long>(rt_grid((int64_t)n + 1), 65536);
+    spmm_csr_t_offsets_kernel<<<grid, RT_THREADS, 0, st>>>(keys, sub, n, (int)nkeys, base, out);
+}
+
+void rt_rows(cudaStream_t st, const int* off, int off_base, int64_t rows, const int* perm, int n, int out_base, int* out) {
+    spmm_csr_t_rows_kernel<<<rt_grid(n), RT_THREADS, 0, st>>>(off, off_base, (int)rows, perm, n, out_base, out);
+}
+
+bool rt_gather(cudaStream_t st, int width, const void* src, const int* perm, int n, void* dst) {
+    const unsigned g = rt_grid(n);
+    switch (width) {
+    case 1: spmm_csr_t_gather_kernel<unsigned char><<<g, RT_THREADS, 0, st>>>((const unsigned char*)src, perm, n, (unsigned char*)dst); break;
+    case 2: spmm_csr_t_gather_kernel<unsigned short><<<g, RT_THREADS, 0, st>>>((const unsigned short*)src, perm, n, (unsigned short*)dst); break;
+    case 4: spmm_csr_t_gather_kernel<unsigned><<<g, RT_THREADS, 0, st>>>((const unsigned*)src, perm, n, (unsigned*)dst); break;
+    case 8: spmm_csr_t_gather_kernel<unsigned long long><<<g, RT_THREADS, 0, st>>>((const unsigned long long*)src, perm, n, (unsigned long long*)dst); break;
+    case 16: spmm_csr_t_gather_kernel<uint4><<<g, RT_THREADS, 0, st>>>((const uint4*)src, perm, n, (uint4*)dst); break;
+    default: return false;
+    }
+    return true;
+}
+
 static size_t elem_bytes(int dtype) { return dtype == T_F64 ? 8 : dtype == T_F32 ? 4 : 2; }
 static bool is16(int dtype) { return dtype == T_F16 || dtype == T_BF16; }
 
 struct TLayout {
-    size_t t_off, t_row, perm, k0, k1, v0, v1, hist, tot, t_val, ws, ws_bytes, total;
+    size_t t_off, t_row, perm, k0, t_val, ws, ws_bytes, total;
 };
 
 static TLayout t_layout(int dtype, int64_t rows, int64_t cols, int64_t n, int64_t nnz, int64_t sbk, int64_t sbj) {
     TLayout L;
-    const size_t e = (size_t)nnz * 4, nt = (size_t)rt_ntiles(nnz);
+    const size_t e = (size_t)nnz * 4;
     L.t_off = 0;
     L.t_row = up256(((size_t)cols + 1) * 4);
     L.perm = L.t_row + up256(e);
     L.k0 = L.perm + up256(e);
-    L.k1 = L.k0 + up256(e);
-    L.v0 = L.k1 + up256(e);
-    L.v1 = L.v0 + up256(e);
-    L.hist = L.v1 + up256(e);
-    L.tot = L.hist + up256((size_t)RT_BINS * nt * 4);
-    L.t_val = L.tot + up256((size_t)RT_BINS * 4);
+    L.t_val = L.k0 + rt_scratch_bytes(nnz);
     L.ws = L.t_val + up256((size_t)nnz * elem_bytes(dtype));
     // the N kernel's workspace for the cols x rows CSR matrix A^T: the row-major copy of a K-contiguous B (and the 16-bit carry slots)
     if (is16(dtype)) L.ws_bytes = b200spmm_csr16_workspace_bytes(rows, n, nnz, sbk, sbj);
@@ -193,32 +248,16 @@ static bool dims_ok(int64_t rows, int64_t cols, int64_t nnz) {
 static int build_plan(cudaStream_t st, int64_t rows, int64_t cols, int64_t nnz, const int* off, const int* col, int base, char* ws) {
     const TLayout L = t_layout(T_F32, rows, cols, 0, nnz, 0, 0);
     int* t_off = (int*)(ws + L.t_off);
+    int* perm = (int*)(ws + L.perm);
     const int nz = (int)nnz;
-    const int* keys = col;
-    const int* vals = nullptr;
-    int sub = base;
     if (nz > 0) {
-        const int ntiles = (int)rt_ntiles(nnz), passes = rt_passes(cols);
-        int* kb[2] = {(int*)(ws + L.k0), (int*)(ws + L.k1)};
-        int* vb[2] = {(int*)(ws + L.v0), (int*)(ws + L.v1)};
-        int* hist = (int*)(ws + L.hist);
-        int* tot = (int*)(ws + L.tot);
-        for (int p = 0; p < passes; p++) {
-            const int shift = p * RT_BITS;
-            int* vo = p == passes - 1 ? (int*)(ws + L.perm) : vb[p & 1];
-            spmm_csr_t_hist_kernel<<<ntiles, RT_THREADS, 0, st>>>(keys, sub, nz, shift, hist, ntiles);
-            spmm_csr_t_scan_kernel<<<RT_BINS, RT_THREADS, 0, st>>>(hist, ntiles, tot);
-            spmm_csr_t_scatter_kernel<<<ntiles, RT_THREADS, 0, st>>>(keys, sub, vals, nz, shift, hist, tot, ntiles, kb[p & 1], vo);
-            keys = kb[p & 1]; vals = vo; sub = 0;
-        }
+        const int* sorted = nullptr;
+        rt_sort(st, col, base, nullptr, nullptr, nz, cols, rt_scratch(ws + L.k0, nnz), perm, &sorted, nullptr);
+        rt_offsets(st, sorted, 0, nz, cols, 0, t_off);
+        rt_rows(st, off, base, rows, perm, nz, 0, (int*)(ws + L.t_row));
+    } else {
+        rt_offsets(st, nullptr, 0, 0, cols, 0, t_off);
     }
-    const long long work = nnz + 1;
-    const unsigned grid = (unsigned)std::min<long long>((work + RT_THREADS - 1) / RT_THREADS, 65536);
-    spmm_csr_t_offsets_kernel<<<grid, RT_THREADS, 0, st>>>(nz > 0 ? keys : nullptr, nz, (int)cols, t_off);
-    if (nz > 0)
-        spmm_csr_t_rows_kernel<<<(unsigned)((nnz + RT_THREADS - 1) / RT_THREADS), RT_THREADS, 0, st>>>(off, base, (int)rows,
-                                                                                                    (const int*)(ws + L.perm), nz,
-                                                                                                    (int*)(ws + L.t_row));
     return (int)cudaGetLastError();
 }
 
@@ -283,10 +322,7 @@ int b200spmm_csr_t(void* stream, int dtype, int c_type, int64_t rows, int64_t co
     const int* perm = (const int*)(ws + L.perm);
     void* t_val = ws + L.t_val;
     if (nnz > 0) {
-        const unsigned g = (unsigned)((nnz + RT_THREADS - 1) / RT_THREADS);
-        if (dtype == T_F64) spmm_csr_t_gather_kernel<unsigned long long><<<g, RT_THREADS, 0, st>>>((const unsigned long long*)values, perm, (int)nnz, (unsigned long long*)t_val);
-        else if (dtype == T_F32) spmm_csr_t_gather_kernel<unsigned><<<g, RT_THREADS, 0, st>>>((const unsigned*)values, perm, (int)nnz, (unsigned*)t_val);
-        else spmm_csr_t_gather_kernel<unsigned short><<<g, RT_THREADS, 0, st>>>((const unsigned short*)values, perm, (int)nnz, (unsigned short*)t_val);
+        rt_gather(st, (int)elem_bytes(dtype), values, perm, (int)nnz, t_val);
         const cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return (int)e;
     }

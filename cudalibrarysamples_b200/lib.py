@@ -117,6 +117,16 @@ def shim(build_if_missing: bool = False) -> C.CDLL:
         lib.b200spmm_csr_t_workspace_bytes.restype = C.c_size_t
         lib.b200spmm_csr_t_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]
         lib.b200spmv_plan_trusted.argtypes = [vp, vp, C.c_int]
+        lib.b200csr2csc.argtypes = [vp, i64, i64, i64, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int32, vp, C.c_size_t]
+        lib.b200csr2csc_workspace_bytes.argtypes = [i64, i64, i64]
+        lib.b200csr2csc_workspace_bytes.restype = C.c_size_t
+        lib.b200coosort.argtypes = [vp, C.c_int, i64, i64, i64, vp, vp, vp, vp, C.c_size_t]
+        lib.b200coosort_workspace_bytes.argtypes = [i64, i64, i64]
+        lib.b200coosort_workspace_bytes.restype = C.c_size_t
+        lib.b200coo2csr.argtypes = [vp, vp, i64, i64, vp, C.c_int32]
+        lib.b200csr2coo.argtypes = [vp, vp, i64, i64, vp, C.c_int32]
+        lib.b200identity_permutation.argtypes = [vp, i64, vp]
+        lib.b200conv_route.argtypes = [C.c_int, i64, i64, i64, C.c_int, C.c_int, vp]
         lib.b200spmv_csr16.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, vp, vp, C.c_size_t]
         lib.b200spmv_csr16_workspace_bytes.argtypes = [i64, i64]
         lib.b200spmv_csr16_workspace_bytes.restype = C.c_size_t

@@ -374,6 +374,32 @@ B200SPMV_EXPORT size_t b200spmm_csr_t_layout(int dtype, int64_t rows, int64_t co
 B200SPMV_EXPORT size_t b200spmm_csr_t_workspace_bytes(int dtype, int64_t rows, int64_t cols, int64_t n, int64_t nnz, int64_t sbk,
                                                       int64_t sbj);
 
+/* Format conversions (convert.cu), int32 indices, on the stable radix sort of the transposed plan: every result is a pure function
+ * of the input, ties included.  Each returns -1 with nothing launched on a bad argument (negative or oversized sizes, a base other
+ * than 0 / 1, a NULL or misaligned array the call needs, a NULL, misaligned or short workspace), else the CUDA launch status.  For
+ * any index values, nothing is written outside the caller's outputs and workspace; out-of-range indices give an undefined result.
+ * No allocation, no host synchronisation: graph-capturable.
+ *
+ * CSR -> CSC (cusparseCsr2cscEx2): A m x n CSR (base 0 or 1) to cscColPtr[n + 1] and cscRowInd[nnz] in the same base and, when
+ * numeric is nonzero, cscVal[nnz] moved bit for bit, value_bytes 1, 2, 4, 8 or 16 wide.  Rows ascend within a column; duplicate
+ * (row, col) entries keep their CSR order; columns need not be sorted within a row.  workspace: b200csr2csc_workspace_bytes()
+ * bytes, 16-byte aligned (may be NULL when nnz = 0). */
+B200SPMV_EXPORT int b200csr2csc(void* stream, int64_t m, int64_t n, int64_t nnz, const void* csr_val, const void* csr_row_ptr,
+                                const void* csr_col_ind, void* csc_val, void* csc_col_ptr, void* csc_row_ind, int value_bytes, int numeric,
+                                int32_t base, void* workspace, size_t workspace_bytes);
+B200SPMV_EXPORT size_t b200csr2csc_workspace_bytes(int64_t m, int64_t n, int64_t nnz);
+/* In-place COO sort (cusparseXcoosortByRow / ByColumn): rows and cols sorted lexicographically by (row, col) when by_row is nonzero,
+ * else by (col, row); equal pairs keep their input order.  P gets the same permutation: P_out[i] = P_in[sigma(i)].  Keys are plain
+ * ints in [0, m] / [0, n], so base 0 and base 1 both sort.  workspace: b200coosort_workspace_bytes() bytes, 16-byte aligned. */
+B200SPMV_EXPORT int b200coosort(void* stream, int by_row, int64_t m, int64_t n, int64_t nnz, void* rows, void* cols, void* P,
+                                void* workspace, size_t workspace_bytes);
+B200SPMV_EXPORT size_t b200coosort_workspace_bytes(int64_t m, int64_t n, int64_t nnz);
+/* cusparseXcoo2csr: csrRowPtr[m + 1] from the sorted cooRowInd[nnz], in the given base.  cusparseXcsr2coo: cooRowInd[nnz], the row
+ * of each entry, from csrRowPtr[m + 1].  cusparseCreateIdentityPermutation: p[i] = i for i < n.  These three need no workspace. */
+B200SPMV_EXPORT int b200coo2csr(void* stream, const void* coo_row_ind, int64_t nnz, int64_t m, void* csr_row_ptr, int32_t base);
+B200SPMV_EXPORT int b200csr2coo(void* stream, const void* csr_row_ptr, int64_t nnz, int64_t m, void* coo_row_ind, int32_t base);
+B200SPMV_EXPORT int b200identity_permutation(void* stream, int64_t n, void* p);
+
 /* The BLAS-1 part of a CG iteration, fused, all scalars in DEVICE memory (no host synchronisation, CUDA-graph capturable).
  * Replaces the cublasDdot / cublasDaxpy / cublasDnrm2 / cublasDscal calls between two cusparseSpMV calls of gpu_CG
  * (cuSPARSE/cg/cg_example.c:226-286).  fp64; vectors 16-byte aligned; `workspace` = b200cg_workspace_bytes() bytes, zeroed
@@ -528,6 +554,18 @@ B200SPMV_EXPORT int b200spmm_csr_t_route(const void* matA, const void* matB, con
  * transposed SpMM plan (cusparseSpMM_preprocess).  A buffer holds the plan of its latest preprocess only, and each kind trusts only
  * its own; cusparseCsrSetPointers, a new bufferSize query of that operation and cusparseDestroySpMat drop the trust.  Host logic only. */
 B200SPMV_EXPORT int b200spmv_plan_trusted(const void* matA, void* buffer, int kind);
+/* Where the shim sends a conversion call: 1 = the native entry point above, 0 = the closed library.  op: B200CONV_CSR2CSC (arg:
+ * value bytes, 0 for CUSPARSE_ACTION_SYMBOLIC), B200CONV_COOSORT_ROW / _COL, B200CONV_COO2CSR, B200CONV_CSR2COO, B200CONV_IDENTITY
+ * (arg unused); alg: cusparseCsr2CscAlg_t (csr2csc only); buffer: the call's buffer (csr2csc with nnz > 0 and coosort only).
+ * Native needs CUSPARSE_CSR2CSC_ALG1, a non-NULL 16-byte aligned buffer where one is used, sizes within the sort's limits, no
+ * B200SPMV_FORWARD=1, and a class measured at least at parity with the closed library (DESIGN.md 3.23).  Host logic only. */
+#define B200CONV_CSR2CSC 0
+#define B200CONV_COOSORT_ROW 1
+#define B200CONV_COOSORT_COL 2
+#define B200CONV_COO2CSR 3
+#define B200CONV_CSR2COO 4
+#define B200CONV_IDENTITY 5
+B200SPMV_EXPORT int b200conv_route(int op, int64_t m, int64_t n, int64_t nnz, int arg, int alg, const void* buffer);
 /* ---------------------------------------------------------------------------------------------- *
  * Sparse triangular solve with many right-hand sides (cusparseSpSM; cuSPARSE/spsm_csr):           *
  *   C = alpha op(T)^-1 op(B), T the selected triangle of the rows x rows CSR matrix A (int32       *
@@ -691,6 +729,18 @@ B200SPMV_EXPORT cusparseStatus_t cusparseSpSM_solve(cusparseHandle_t, cusparseOp
                                                     cusparseConstSpMatDescr_t, cusparseConstDnMatDescr_t, cusparseDnMatDescr_t,
                                                     cudaDataType, cusparseSpSMAlg_t, cusparseSpSMDescr_t);
 B200SPMV_EXPORT cusparseStatus_t cusparseSpSM_updateMatrix(cusparseHandle_t, cusparseSpSMDescr_t, void*, cusparseSpSMUpdate_t);
+/* cusparse.h:3263-3276, 4099-4130, 4951-4982 -- coosort_example.c */
+B200SPMV_EXPORT cusparseStatus_t cusparseCsr2cscEx2_bufferSize(cusparseHandle_t, int, int, int, const void*, const int*, const int*, void*,
+                                                               int*, int*, cudaDataType, cusparseAction_t, cusparseIndexBase_t,
+                                                               cusparseCsr2CscAlg_t, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseCsr2cscEx2(cusparseHandle_t, int, int, int, const void*, const int*, const int*, void*, int*, int*,
+                                                    cudaDataType, cusparseAction_t, cusparseIndexBase_t, cusparseCsr2CscAlg_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseXcoosort_bufferSizeExt(cusparseHandle_t, int, int, int, const int*, const int*, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseXcoosortByRow(cusparseHandle_t, int, int, int, int*, int*, int*, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseXcoosortByColumn(cusparseHandle_t, int, int, int, int*, int*, int*, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseXcoo2csr(cusparseHandle_t, const int*, int, int, int*, cusparseIndexBase_t);
+B200SPMV_EXPORT cusparseStatus_t cusparseXcsr2coo(cusparseHandle_t, const int*, int, int, int*, cusparseIndexBase_t);
+B200SPMV_EXPORT cusparseStatus_t cusparseCreateIdentityPermutation(cusparseHandle_t, int, int*);
 #ifdef __cplusplus
 }
 #endif
