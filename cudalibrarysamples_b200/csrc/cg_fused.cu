@@ -16,6 +16,7 @@
 // order.  fp64 only (the solvers of the reference are fp64: cg_example.c:311, bicgstab_example.c:375).
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "spmv_common.cuh"
 #include "../../include/b200spmv.h"
 
 namespace b200cg {
@@ -25,8 +26,7 @@ constexpr int MAX_CTAS = 132 * 16;   // 256 threads x 16 CTAs/SM candidates: ple
 
 // workspace: [0 .. MAX_CTAS) partial sums, then one arrival counter (as a double slot)
 __device__ __forceinline__ double block_sum(double v, double* sred) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    v = b200::warp_allsum(v);
     if ((threadIdx.x & 31) == 0) sred[threadIdx.x >> 5] = v;
     __syncthreads();
     double t = 0;

@@ -13,6 +13,7 @@
 // Whatever the indices hold, nothing is written outside the caller's outputs and workspace; the result of out-of-range input is
 // undefined.  No allocation, no host synchronisation: graph-capturable.
 #include "radix_sort.cuh"
+#include "spmv_common.cuh"
 #include "../../include/b200spmv.h"
 
 #include <algorithm>
@@ -23,7 +24,6 @@ __global__ void __launch_bounds__(RT_THREADS) identity_permutation_kernel(int* p
     for (long long i = (long long)blockIdx.x * RT_THREADS + threadIdx.x; i < n; i += (long long)gridDim.x * RT_THREADS) p[i] = (int)i;
 }
 
-static size_t up256(size_t b) { return (b + 255) / 256 * 256; }
 static bool aligned(const void* p, size_t a) { return ((uintptr_t)p & (a - 1)) == 0; }
 static bool width_ok(int w) { return w == 1 || w == 2 || w == 4 || w == 8 || w == 16; }
 
@@ -71,7 +71,7 @@ int b200csr2csc(void* stream, int64_t m, int64_t n, int64_t nnz, const void* csr
 
 size_t b200coosort_workspace_bytes(int64_t m, int64_t n, int64_t nnz) {
     if (!conv_dims_ok(m, n, nnz)) return 0;
-    return rt_scratch_bytes(nnz) + up256((size_t)nnz * 4);
+    return rt_scratch_bytes(nnz) + round_up_256((size_t)nnz * 4);
 }
 
 int b200coosort(void* stream, int by_row, int64_t m, int64_t n, int64_t nnz, void* rows, void* cols, void* P, void* workspace,

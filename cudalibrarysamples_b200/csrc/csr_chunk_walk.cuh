@@ -56,17 +56,6 @@ __device__ __forceinline__ int csr_first_row(const Args& a, int e) {
     return lo;
 }
 
-// the row holding entry e < nnz: the last r with off[r] <= e
-template <class Args>
-__device__ __forceinline__ int csr_last_row(const Args& a, int e) {
-    int lo = 0, hi = a.rows;
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (csr_off(a, mid) <= e) lo = mid; else hi = mid;
-    }
-    return lo;
-}
-
 // S of the piece [s, e) (chunk coordinates): 0 + its runs' sums in ascending order; a run covered in part adds 0 + its products in order
 template <class P>
 __device__ __forceinline__ typename P::Acc csr_walk_piece(const typename P::Acc* prod, const typename P::Acc* runs, int s, int e) {
@@ -153,7 +142,7 @@ __device__ __forceinline__ void csr_walk_fixup(const typename P::Args a, const S
     const int c = (int)blockIdx.x * CSR_WALK_FIXUP_THREADS + (int)threadIdx.x;
     if (c >= a.nchunks - 1) return;
     const int cs = c * P::CHUNK, ce = cs + P::CHUNK;
-    const int r = csr_last_row(a, ce - 1);              // the row holding the chunk's last entry (< nnz)
+    const int r = csr_row_of(a.off, a.rows, a.base, ce - 1);   // the row holding the chunk's last entry (< nnz)
     const int rs = csr_off(a, r), re = csr_off(a, r + 1);
     if (rs < cs || re <= ce) return;                    // it starts before the chunk, or ends in it
     typename P::Acc acc = P::add(P::zero(), a.carry[2 * c + 1]);
@@ -176,8 +165,8 @@ static size_t csr_walk_carry_bytes(int64_t rows, int64_t nnz) {
 // same bits.  One chunk: no row leaves it.
 template <int E, typename Acc>
 static Acc* csr_walk_carry(int64_t rows, int64_t nnz, void* workspace, size_t workspace_bytes) {
-    const bool split = csr_walk_nchunks<E>(nnz) > 1 && workspace && ((uintptr_t)workspace & 15) == 0 &&
-                       workspace_bytes >= csr_walk_carry_bytes<E, Acc>(rows, nnz);
+    const bool split = csr_walk_nchunks<E>(nnz) > 1 &&
+                       workspace_usable(workspace, workspace_bytes, csr_walk_carry_bytes<E, Acc>(rows, nnz));
     return split ? (Acc*)workspace : nullptr;
 }
 

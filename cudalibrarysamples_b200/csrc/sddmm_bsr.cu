@@ -47,21 +47,6 @@ struct BsrArgs {
     int        tiles;                                               // tiles per block side
 };
 
-__device__ __forceinline__ float to_acc(__half v) { return __half2float(v); }
-__device__ __forceinline__ float to_acc(__nv_bfloat16 v) { return __bfloat162float(v); }
-__device__ __forceinline__ float to_acc(float v) { return v; }
-__device__ __forceinline__ double to_acc(double v) { return v; }
-
-// block-row of stored block e: the last r with off[r] - base <= e (off[0] - base = 0 <= e < off[brows] - base = bnnz)
-__device__ __forceinline__ int bsr_block_row(const int* off, int brows, int base, int e) {
-    int lo = 0, hi = brows;
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (__ldg(off + mid) - base <= e) lo = mid; else hi = mid;
-    }
-    return lo;
-}
-
 // C entry = alpha * acc + beta * C entry, rounded once to C's type (T, or fp32 when c_f32)
 template <typename T, typename S>
 __device__ __forceinline__ void bsr_store(void* V, long long o, bool c_f32, S acc, S alpha, S beta) {
@@ -98,7 +83,7 @@ __global__ void __launch_bounds__(TILE == 16 ? 32 : 128) sddmm_bsr_mma_kernel(co
     const int tiles2 = a.tiles * a.tiles;
     const int e = (int)(blockIdx.x / tiles2), t = (int)(blockIdx.x % tiles2);
     const long long bi = blockIdx.y;
-    const int br = bsr_block_row(a.off + bi * a.off_stride, a.brows, a.base, e);
+    const int br = csr_row_of(a.off + bi * a.off_stride, a.brows, a.base, e);
     const int bc = __ldg(a.col + bi * a.col_stride + e) - a.base;
     const int ti = (t / a.tiles) * TILE, tj = (t % a.tiles) * TILE;     // the tile inside the block
     const long long r0 = (long long)br * a.bs + ti, c0 = (long long)bc * a.bs + tj;
@@ -207,7 +192,7 @@ __global__ void __launch_bounds__(BSR_FMA_THREADS) sddmm_bsr_fma_kernel(const Bs
     if (slot >= BSR_FMA_THREADS / tpt || g >= (long long)a.bnnz * tiles2) return;
     const int e = (int)(g / tiles2), t = (int)(g % tiles2);
     const long long bi = blockIdx.y;
-    const int br = bsr_block_row(a.off + bi * a.off_stride, a.brows, a.base, e);
+    const int br = csr_row_of(a.off + bi * a.off_stride, a.brows, a.base, e);
     const int bc = __ldg(a.col + bi * a.col_stride + e) - a.base;
     const int i0 = (t / a.tiles) * st + (w / per) * MR, j0 = (t % a.tiles) * st + (w % per) * MR;   // inside the block
     const T* pa = (const T*)a.A + bi * a.a_stride + ((long long)br * a.bs + i0) * a.sai;
@@ -242,14 +227,6 @@ __global__ void __launch_bounds__(BSR_FMA_THREADS) sddmm_bsr_fma_kernel(const Bs
                 const long long o = a.c_row ? (long long)(i0 + r) * a.bs + j0 + c : (long long)(j0 + c) * a.bs + i0 + r;
                 bsr_store<T>(a.val, vbase + o, a.c_f32, acc[r][c], alpha, beta);
             }
-}
-
-template <typename S>
-static Scalars<S> bsr_scalars(const void* alpha, const void* beta, int on_device) {
-    Scalars<S> s;
-    if (on_device) { s.alpha = S(0); s.beta = S(0); s.alpha_dev = (const S*)alpha; s.beta_dev = (const S*)beta; }
-    else { s.alpha = *(const S*)alpha; s.beta = *(const S*)beta; s.alpha_dev = nullptr; s.beta_dev = nullptr; }
-    return s;
 }
 
 template <typename T>
@@ -336,8 +313,13 @@ int b200sddmm_bsr(void* stream, int ab_type, int c_type, int64_t m, int64_t n, i
     a.brows = (int)(m / bs); a.bnnz = (int)bnnz; a.bs = (int)bs; a.k = (int)k; a.base = base; a.c_row = c_row_major != 0;
     a.c_f32 = h16 && c_type == DT_F32; a.tiles = 1;
     const cudaStream_t st = (cudaStream_t)stream;
-    if (ab_type == DT_F64) return launch_bsr_fma<double, double>(st, a, bsr_scalars<double>(alpha, beta, scalars_on_device), batch);
-    const Scalars<float> sc = bsr_scalars<float>(alpha, beta, scalars_on_device);
+    if (ab_type == DT_F64) {
+        Scalars<double> sd;
+        set_scalars(sd, alpha, beta, scalars_on_device);
+        return launch_bsr_fma<double, double>(st, a, sd, batch);
+    }
+    Scalars<float> sc;
+    set_scalars(sc, alpha, beta, scalars_on_device);
     if (ab_type == DT_F32) return launch_bsr_fma<float, float>(st, a, sc, batch);
     if (b200sddmm_bsr_path(ab_type, bs, A, sai, sak, B, sbk, sbj, batch, a_stride, b_stride)) {
         const bool ak = sak == 1 && sai % 8 == 0, bk = sbk == 1 && sbj % 8 == 0;

@@ -70,7 +70,8 @@ __global__ void __launch_bounds__(32 * SDDMM_WARPS) sddmm_csr_kernel(const Sddmm
     T*         val = a.val + bi * a.cv_stride;
     const T*   A = a.A + bi * a.a_stride;
     const T*   B = a.B + bi * a.b_stride;
-    // row of entry n0: the last r with off[r] - base <= n0 (invariant off[lo] - base <= n0 < off[hi] - base, off[rows] = nnz)
+    // row of entry n0: the last r with off[r] - base <= n0 (invariant off[lo] - base <= n0 < off[hi] - base, off[rows] = nnz).
+    // Not csr_row_of: as a call, a.base is loaded ahead of the search and the kernel compiles to different SASS.
     int lo = 0, hi = a.rows;
     while (hi - lo > 1) {
         const int mid = (lo + hi) >> 1;
@@ -129,8 +130,6 @@ struct SddmmCopies {
     size_t a_bytes = 0, b_bytes = 0;
 };
 
-static size_t round256(size_t x) { return (x + 255) / 256 * 256; }
-
 static SddmmCopies sddmm_copies(int dtype, int64_t m, int64_t n, int64_t k, int64_t sai, int64_t sak, int64_t sbk, int64_t sbj, int batch,
                                 int64_t a_stride, int64_t b_stride) {
     SddmmCopies c;
@@ -138,11 +137,11 @@ static SddmmCopies sddmm_copies(int dtype, int64_t m, int64_t n, int64_t k, int6
     const int64_t kmax = 32LL * 65535;                           // grid.y of spmm_transpose_b_kernel
     if (k > 1 && k <= kmax && sak != 1 && sai == 1 && m > 0) {
         c.a = true;
-        c.a_bytes = round256((size_t)(batch > 1 && a_stride != 0 ? batch : 1) * (size_t)m * (size_t)k * vsz);
+        c.a_bytes = round_up_256((size_t)(batch > 1 && a_stride != 0 ? batch : 1) * (size_t)m * (size_t)k * vsz);
     }
     if (k > 1 && k <= kmax && sbk != 1 && sbj == 1 && n > 0) {
         c.b = true;
-        c.b_bytes = round256((size_t)(batch > 1 && b_stride != 0 ? batch : 1) * (size_t)n * (size_t)k * vsz);
+        c.b_bytes = round_up_256((size_t)(batch > 1 && b_stride != 0 ? batch : 1) * (size_t)n * (size_t)k * vsz);
     }
     return c;
 }
@@ -162,7 +161,7 @@ static int launch_sddmm(cudaStream_t stream, int64_t m, int64_t n, int64_t k, in
     if (k <= 1) { sak = 1; sbk = 1; }                            // a single k: its stride is never used
     if (batch == 1) { off_stride = cv_stride = a_stride = b_stride = 0; }
     const SddmmCopies cp = sddmm_copies(sizeof(T) == 8 ? 1 : 0, m, n, k, sai, sak, sbk, sbj, batch, a_stride, b_stride);
-    if ((cp.a || cp.b) && ws && ((uintptr_t)ws & 15) == 0 && ws_bytes >= cp.a_bytes + cp.b_bytes) {
+    if ((cp.a || cp.b) && workspace_usable(ws, ws_bytes, cp.a_bytes + cp.b_bytes)) {
         const int dt = sizeof(T) == 8 ? 1 : 0;
         if (cp.a) {
             const int cnt = a_stride != 0 ? batch : 1;
@@ -190,8 +189,7 @@ static int launch_sddmm(cudaStream_t stream, int64_t m, int64_t n, int64_t k, in
     a.base = base; a.rows = (int)m; a.nnz = (int)nnz; a.k = (int)k; a.lg = group_log2(k, vec ? VW : 1);
     a.sai = sai; a.sak = sak; a.sbk = sbk; a.sbj = sbj;
     a.off_stride = off_stride; a.cv_stride = cv_stride; a.a_stride = a_stride; a.b_stride = b_stride;
-    if (on_device) { a.s.alpha = T(0); a.s.beta = T(0); a.s.alpha_dev = (const T*)alpha; a.s.beta_dev = (const T*)beta; }
-    else { a.s.alpha = *(const T*)alpha; a.s.beta = *(const T*)beta; a.s.alpha_dev = nullptr; a.s.beta_dev = nullptr; }
+    set_scalars(a.s, alpha, beta, on_device);
     const int64_t per_cta = (int64_t)SDDMM_CHUNK * SDDMM_WARPS;
     const dim3 grid((unsigned)((nnz + per_cta - 1) / per_cta), (unsigned)batch);
     if (vec) sddmm_csr_kernel<T, VW><<<grid, 32 * SDDMM_WARPS, 0, stream>>>(a);

@@ -51,9 +51,6 @@ struct BellArgs {
     Scalars<float> s;
 };
 
-__device__ __forceinline__ float to_f(__half v) { return __half2float(v); }
-__device__ __forceinline__ float to_f(__nv_bfloat16 v) { return __bfloat162float(v); }
-
 // C(i, j) = alpha * acc + beta * C(i, j), rounded once to C's type
 template <typename T>
 __device__ __forceinline__ void bell_store(const BellArgs& a, long long i, long long j, float acc, float alpha, float beta) {
@@ -63,7 +60,7 @@ __device__ __forceinline__ void bell_store(const BellArgs& a, long long i, long 
         *p = beta == 0.f ? alpha * acc : alpha * acc + beta * *p;
     } else {
         T* p = (T*)a.C + o;
-        const float v = beta == 0.f ? alpha * acc : alpha * acc + beta * to_f(*p);
+        const float v = beta == 0.f ? alpha * acc : alpha * acc + beta * to_acc(*p);
         if constexpr (std::is_same<T, __half>::value) *p = __float2half_rn(v);
         else *p = __float2bfloat16_rn(v);
     }
@@ -88,7 +85,7 @@ __global__ void __launch_bounds__(BELL_SC_X * BELL_SC_Y) bell_scalar_kernel(cons
         if (c == -1) continue;
         const T* ap = av + (long long)e * a.bs;
         const T* bp = B + (long long)(c - a.base) * a.bs * sk + j * sj;
-        for (int q = 0; q < a.bs; q++) acc = fmaf(to_f(ap[q]), to_f(bp[q * sk]), acc);
+        for (int q = 0; q < a.bs; q++) acc = fmaf(to_acc(ap[q]), to_acc(bp[q * sk]), acc);
     }
     bell_store<T>(a, i, j, acc, a.s.a(), a.s.b());
 }
@@ -256,8 +253,7 @@ int b200spmm_bell(void* stream, int a_type, int c_type, int64_t rows, int64_t co
     a.ell_cols = ell_cols; a.ldb = ldb; a.ldc = ldc;
     a.rows = (int)rows; a.n = (int)n; a.bs = (int)bs; a.eb = (int)(ell_cols / bs); a.base = base;
     a.c_f32 = c_type == DT_F32; a.b_row = b_row_major != 0; a.c_row = c_row_major != 0;
-    if (scalars_on_device) { a.s.alpha = 0.f; a.s.beta = 0.f; a.s.alpha_dev = (const float*)alpha; a.s.beta_dev = (const float*)beta; }
-    else { a.s.alpha = *(const float*)alpha; a.s.beta = *(const float*)beta; a.s.alpha_dev = nullptr; a.s.beta_dev = nullptr; }
+    set_scalars(a.s, alpha, beta, scalars_on_device);
     // the 16-byte cp.async of the tensor path needs aligned panels of A and B; every other operand takes the scalar path
     const bool tensor = bs % BELL_KS == 0 && ((uintptr_t)values & 15) == 0 && ((uintptr_t)B & 15) == 0 && ldb % 8 == 0;
     if (a_type == DT_F16) return launch_bell<__half>((cudaStream_t)stream, a, tensor);

@@ -62,25 +62,10 @@ struct SpmmBsrArgs {
     int         ntiles;                 // column tiles of C per block-row tile
 };
 
-__device__ __forceinline__ float mm_acc(__half v) { return __half2float(v); }
-__device__ __forceinline__ float mm_acc(__nv_bfloat16 v) { return __bfloat162float(v); }
-__device__ __forceinline__ float mm_acc(float v) { return v; }
-__device__ __forceinline__ double mm_acc(double v) { return v; }
-
-// block-row of stored block e < bnnz: the last r with off[r] - base <= e (an empty block-row never contains e)
-__device__ __forceinline__ int mm_block_row(const int* off, int brows, int base, int e) {
-    int lo = 0, hi = brows;
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (__ldg(off + mid) - base <= e) lo = mid; else hi = mid;
-    }
-    return lo;
-}
-
 // the first piece boundary at or after stored block x: a block-row start, or a block-row start plus a multiple of ch
 __device__ __forceinline__ int mm_cut_ge(const SpmmBsrArgs& a, const int* off, int x) {
     if (x >= a.bnnz) return a.bnnz;
-    const int r = mm_block_row(off, a.brows, a.base, x);
+    const int r = csr_row_of(off, a.brows, a.base, x);
     const int rs = __ldg(off + r) - a.base, re = __ldg(off + r + 1) - a.base;
     const long long c = rs + (long long)((x - rs + a.ch - 1) / a.ch) * a.ch;
     return (int)(c < re ? c : re);
@@ -90,7 +75,7 @@ __device__ __forceinline__ int mm_cut_ge(const SpmmBsrArgs& a, const int* off, i
 struct MmWalk {
     int r, rs, re, ps;
     __device__ __forceinline__ void at(const SpmmBsrArgs& a, const int* off, int e) {
-        r = mm_block_row(off, a.brows, a.base, e);
+        r = csr_row_of(off, a.brows, a.base, e);
         rs = __ldg(off + r) - a.base; re = __ldg(off + r + 1) - a.base; ps = e;
     }
     // does stored block e end a piece?
@@ -135,7 +120,7 @@ __device__ __forceinline__ void mm_store(const SpmmBsrArgs& a, long long bi, lon
         *p = beta == S(0) ? alpha * acc : alpha * acc + beta * *p;
     } else {
         T* p = (T*)a.C + o;
-        const float v = beta == S(0) ? alpha * acc : alpha * acc + beta * mm_acc(*p);
+        const float v = beta == S(0) ? alpha * acc : alpha * acc + beta * to_acc(*p);
         if constexpr (std::is_same<T, __half>::value) *p = __float2half_rn(v);
         else if constexpr (std::is_same<T, __nv_bfloat16>::value) *p = __float2bfloat16_rn(v);
     }
@@ -327,10 +312,10 @@ __global__ void __launch_bounds__(SPMM_BSR_FX * SPMM_BSR_FY, 1) spmm_bsr_fma_ker
         const T* blk = V + (long long)e * a.bs * a.bs + (long long)(ti + ty) * ri;
         const T* pb = B + (long long)(__ldg(col + e) - a.base) * a.bs * a.sbk + (long long)j * a.sbj;
         for (int k = 0; k < a.bs; k++) {
-            const S b = jin ? S(mm_acc(__ldg(pb + (long long)k * a.sbk))) : S(0);
+            const S b = jin ? S(to_acc(__ldg(pb + (long long)k * a.sbk))) : S(0);
 #pragma unroll
             for (int m = 0; m < SPMM_BSR_FMR; m++) {
-                const S x = rin[m] ? S(mm_acc(__ldg(blk + (long long)m * SPMM_BSR_FY * ri + k * rk))) : S(0);
+                const S x = rin[m] ? S(to_acc(__ldg(blk + (long long)m * SPMM_BSR_FY * ri + k * rk))) : S(0);
                 acc[m] = fma(x, b, acc[m]);
             }
         }
@@ -394,14 +379,6 @@ static size_t mm_workspace(int ab_type, int64_t m, int64_t n, int64_t bs, int64_
     const double est = 2.0 * (double)mm_nchunks(bnnz, ch) * (double)bs * (double)n * (ab_type == MM_F64 ? 8.0 : 4.0) * batch;
     if (est > 9.0e18) return SIZE_MAX;
     return (size_t)est;
-}
-
-template <typename S>
-static Scalars<S> mm_scalars(const void* alpha, const void* beta, int on_device) {
-    Scalars<S> s;
-    if (on_device) { s.alpha = S(0); s.beta = S(0); s.alpha_dev = (const S*)alpha; s.beta_dev = (const S*)beta; }
-    else { s.alpha = *(const S*)alpha; s.beta = *(const S*)beta; s.alpha_dev = nullptr; s.beta_dev = nullptr; }
-    return s;
 }
 
 template <typename T, int BM, int BN, bool BK>
@@ -514,10 +491,15 @@ int b200spmm_bsr(void* stream, int ab_type, int c_type, int64_t m, int64_t k, in
     a.a_row = a_row_major != 0; a.c_row = c_row_major != 0; a.c_f32 = h16 && c_type == MM_F32; a.ntiles = 1;
     // the split walk needs the carry slots in the caller's buffer; a NULL, misaligned or small buffer gets the unsplit walk
     const size_t need = mm_workspace(ab_type, m, n, bs, bnnz, batch);
-    if (need > 0 && need != SIZE_MAX && workspace && ((uintptr_t)workspace & 15) == 0 && workspace_bytes >= need) a.carry = workspace;
+    if (need > 0 && need != SIZE_MAX && workspace_usable(workspace, workspace_bytes, need)) a.carry = workspace;
     const cudaStream_t st = (cudaStream_t)stream;
-    if (ab_type == MM_F64) return launch_mm<double, double>(st, a, mm_scalars<double>(alpha, beta, scalars_on_device), false, false, batch);
-    const Scalars<float> sc = mm_scalars<float>(alpha, beta, scalars_on_device);
+    if (ab_type == MM_F64) {
+        Scalars<double> sd;
+        set_scalars(sd, alpha, beta, scalars_on_device);
+        return launch_mm<double, double>(st, a, sd, false, false, batch);
+    }
+    Scalars<float> sc;
+    set_scalars(sc, alpha, beta, scalars_on_device);
     if (ab_type == MM_F32) return launch_mm<float, float>(st, a, sc, false, false, batch);
     const bool tensor = b200spmm_bsr_path(ab_type, bs, a_row_major, values, B, sbk, sbj, batch, val_stride, b_stride) == 1;
     const bool bk = sbk == 1 && sbj % 8 == 0;

@@ -255,8 +255,6 @@ __global__ void __launch_bounds__(32 * COO_MM_WARPS) spmm_coo_atomic_kernel(cons
     }
 }
 
-static size_t round256(size_t x) { return (x + 255) / 256 * 256; }
-
 // Workspace layout: [flags: int per batch | carry rows: 2 ints per chunk and batch | carry values: 2 x 64 per chunk, panel and
 // batch | row-major copy of B (one per batch matrix of B)].  SIZE_MAX when the size does not fit a size_t.
 struct CooMmLayout {
@@ -274,10 +272,10 @@ static CooMmLayout coo_mm_layout(int dtype, int64_t kdim, int64_t n, int64_t nnz
     if (est > 9.0e18) { l.total = SIZE_MAX; return l; }
     const size_t nc = (size_t)nchunks, np = (size_t)npanels;
     l.flags = 0;
-    l.carry_row = round256((size_t)batch * 4);
-    l.carry_val = l.carry_row + round256((size_t)batch * nc * 2 * 4);
-    l.bcopy = l.carry_val + round256((size_t)batch * nc * np * 2 * COO_MM_PANEL * vsz);
-    l.total = l.bcopy + (l.copy_b ? round256((size_t)nb * (size_t)kdim * (size_t)n * vsz) : 0);
+    l.carry_row = round_up_256((size_t)batch * 4);
+    l.carry_val = l.carry_row + round_up_256((size_t)batch * nc * 2 * 4);
+    l.bcopy = l.carry_val + round_up_256((size_t)batch * nc * np * 2 * COO_MM_PANEL * vsz);
+    l.total = l.bcopy + (l.copy_b ? round_up_256((size_t)nb * (size_t)kdim * (size_t)n * vsz) : 0);
     return l;
 }
 
@@ -290,7 +288,7 @@ static int launch_coo_mm(cudaStream_t stream, int transpose, int64_t rows, int64
     if (transpose) { std::swap(row_ind, col_ind); std::swap(rows, cols); }   // A^T: the same entries with the index arrays swapped
     if (batch == 1) a_stride = b_stride = c_stride = 0;
     const CooMmLayout l = coo_mm_layout(dt, cols, n, nnz, b_row_major, batch, b_stride);
-    const bool ws_ok = ws && ((uintptr_t)ws & 15) == 0 && l.total != SIZE_MAX && ws_bytes >= l.total;
+    const bool ws_ok = l.total != SIZE_MAX && workspace_usable(ws, ws_bytes, l.total);
     const bool atomic_only = transpose || !ws_ok;
     CooMmArgs<T> a;
     a.row = (const int*)row_ind; a.col = (const int*)col_ind; a.val = (const T*)values; a.B = (const T*)B; a.C = (T*)C;
@@ -308,8 +306,7 @@ static int launch_coo_mm(cudaStream_t stream, int transpose, int64_t rows, int64
     }
     a.sbk = b_row_major ? ldb : 1; a.sbj = b_row_major ? 1 : ldb;
     a.sci = c_row_major ? ldc : 1; a.scj = c_row_major ? 1 : ldc;
-    if (on_device) { a.s.alpha = T(0); a.s.beta = T(0); a.s.alpha_dev = (const T*)alpha; a.s.beta_dev = (const T*)beta; }
-    else { a.s.alpha = *(const T*)alpha; a.s.beta = *(const T*)beta; a.s.alpha_dev = nullptr; a.s.beta_dev = nullptr; }
+    set_scalars(a.s, alpha, beta, on_device);
     a.flags = nullptr; a.carry_row = nullptr; a.carry_val = nullptr;
     const long long cells = rows * n;
     const dim3 sgrid((unsigned)std::max<long long>(1, std::min<long long>((cells + 255) / 256, COO_MM_STRIDE_CTAS)), 1, (unsigned)batch);

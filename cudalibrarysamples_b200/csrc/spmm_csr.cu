@@ -146,8 +146,7 @@ static int launch_spmm(cudaStream_t stream, int64_t rows, int64_t n, const void*
     }
     a.sbk = b_row_major ? ldb : 1; a.sbj = b_row_major ? 1 : ldb;
     a.sci = c_row_major ? ldc : 1; a.scj = c_row_major ? 1 : ldc;
-    if (on_device) { a.s.alpha = T(0); a.s.beta = T(0); a.s.alpha_dev = (const T*)alpha; a.s.beta_dev = (const T*)beta; }
-    else { a.s.alpha = *(const T*)alpha; a.s.beta = *(const T*)beta; a.s.alpha_dev = nullptr; a.s.beta_dev = nullptr; }
+    set_scalars(a.s, alpha, beta, on_device);
     if (!c_row_major && b_row_major) {               // column-major C from row-major B: tiles of C transposed in shared memory
         const dim3 grid((unsigned)((rows + SPMM_TILE_ROWS - 1) / SPMM_TILE_ROWS), (unsigned)((n + SPMM_PANEL - 1) / SPMM_PANEL));
         spmm_csr_ctile_kernel<T><<<grid, 32 * SPMM_WARPS, 0, stream>>>(a);
@@ -166,7 +165,7 @@ extern "C" {
 
 size_t b200spmm_csr_workspace_bytes(int dtype, int64_t cols, int64_t n, int b_row_major) {
     if (b_row_major || n < SPMM_MIN_N_FOR_TRANSPOSE || cols <= 0 || n <= 0) return 0;
-    return ((size_t)cols * (size_t)n * (dtype == 1 ? 8 : 4) + 255) / 256 * 256;
+    return round_up_256((size_t)cols * (size_t)n * (dtype == 1 ? 8 : 4));
 }
 
 int b200spmm_csr_ws(void* stream, int dtype, int64_t rows, int64_t cols, int64_t n, int64_t nnz, const void* row_offsets,

@@ -57,19 +57,6 @@ struct SpmmCsr16Args {
     int         c_f32;                  // C is fp32 (else A's type)
 };
 
-__device__ __forceinline__ float h2f(__half v) { return __half2float(v); }
-__device__ __forceinline__ float h2f(__nv_bfloat16 v) { return __bfloat162float(v); }
-
-// the row holding entry x < nnz: the last r with off[r] - base <= x (an empty row never holds x)
-__device__ __forceinline__ int csr16_row(const SpmmCsr16Args& a, int x) {
-    int lo = 0, hi = a.rows;
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (__ldg(a.off + mid) - a.base <= x) lo = mid; else hi = mid;
-    }
-    return lo;
-}
-
 // C entry (i, j) = alpha * acc + beta * C in fp32, rounded once to C's type
 template <typename T>
 __device__ __forceinline__ void csr16_store(const SpmmCsr16Args& a, bool c_row, long long i, long long j, float acc, float alpha,
@@ -80,7 +67,7 @@ __device__ __forceinline__ void csr16_store(const SpmmCsr16Args& a, bool c_row, 
         *p = beta == 0.f ? __fmul_rn(alpha, acc) : __fmaf_rn(alpha, acc, __fmul_rn(beta, *p));
     } else {
         T* p = (T*)a.C + o;
-        const float v = beta == 0.f ? __fmul_rn(alpha, acc) : __fmaf_rn(alpha, acc, __fmul_rn(beta, h2f(*p)));
+        const float v = beta == 0.f ? __fmul_rn(alpha, acc) : __fmaf_rn(alpha, acc, __fmul_rn(beta, to_acc(*p)));
         if constexpr (std::is_same<T, __half>::value) *p = __float2half_rn(v);
         else *p = __float2bfloat16_rn(v);
     }
@@ -117,7 +104,7 @@ __device__ __forceinline__ void csr16_piece(const SpmmCsr16Args& a, int s, int e
     for (int p = s; p < e; p += SPMM_CSR16_LANE_ENTRIES) {
         const int i = p + lane;
         const int c = i < e ? ldg_stream(a.col + i) - a.base : 0;
-        const float v = i < e ? h2f(vals[i]) : 0.f;
+        const float v = i < e ? to_acc(vals[i]) : 0.f;
         const int cnt = min(SPMM_CSR16_LANE_ENTRIES, e - p);
         for (int t = 0; t < cnt; t += U) {
             int kk[U];
@@ -135,7 +122,7 @@ __device__ __forceinline__ void csr16_piece(const SpmmCsr16Args& a, int s, int e
             for (int u = 0; u < U; u++)
                 if (jin && t + u < cnt) {
 #pragma unroll
-                    for (int q = 0; q < V; q++) acc[q] = __fmaf_rn(vv[u], h2f(h[u][q]), acc[q]);
+                    for (int q = 0; q < V; q++) acc[q] = __fmaf_rn(vv[u], to_acc(h[u][q]), acc[q]);
                 }
         }
     }
@@ -167,7 +154,7 @@ __global__ void __launch_bounds__(32 * SPMM_CSR16_WARPS) spmm_csr16_kernel(const
         const int c = ((int)blockIdx.x - a.ntiles) * SPMM_CSR16_WARPS + warp;
         if (c >= a.nchunks) return;
         const int x = c * P;
-        const int r = csr16_row(a, x);
+        const int r = csr_row_of(a.off, a.rows, a.base, x);
         const int rs = __ldg(a.off + r) - a.base, re = __ldg(a.off + r + 1) - a.base;
         if (re - rs <= P) return;
         const int ps = rs + ((x - rs + P - 1) / P) * P;   // x <= ps < x + P
@@ -239,7 +226,7 @@ __global__ void __launch_bounds__(32 * SPMM_CSR16_WARPS) spmm_csr16_fixup_kernel
     const int c = (int)blockIdx.x * SPMM_CSR16_WARPS + ((int)threadIdx.x >> 5);
     if (c >= a.nchunks) return;
     const long long last = min((long long)(c + 1) * P, (long long)a.nnz) - 1;
-    const int r = csr16_row(a, (int)last);
+    const int r = csr_row_of(a.off, a.rows, a.base, (int)last);
     const int rs = __ldg(a.off + r) - a.base, re = __ldg(a.off + r + 1) - a.base;
     if (rs < c * P || re - rs <= P) return;
     const float alpha = sc.a(), beta = sc.b();
@@ -256,7 +243,7 @@ static int csr16_v(int64_t n) { return n <= 32 ? 1 : n <= 64 ? 2 : n <= 128 ? 4 
 static int64_t csr16_nchunks(int64_t nnz) { return (nnz + SPMM_CSR16_PIECE - 1) / SPMM_CSR16_PIECE; }
 // a K-contiguous op(B) is read through a row-major copy in the workspace
 static bool csr16_copy(int64_t n, int64_t sbk, int64_t sbj) { return n >= 2 && sbk == 1 && sbj != 1; }
-static size_t csr16_copy_bytes(int64_t k, int64_t n) { return ((size_t)k * (size_t)n * 2 + 255) / 256 * 256; }
+static size_t csr16_copy_bytes(int64_t k, int64_t n) { return round_up_256((size_t)k * (size_t)n * 2); }
 
 static int csr16_path(int64_t n, const void* B, int64_t sbk, int64_t sbj) {
     const int v = csr16_v(n);
@@ -342,13 +329,12 @@ int b200spmm_csr16(void* stream, int ab_type, int c_type, int64_t m, int64_t k, 
     a.rows = (int)m; a.n = (int)n; a.nnz = (int)nnz; a.base = base; a.nchunks = (int)csr16_nchunks(nnz); a.ntiles = 0;
     a.c_f32 = c_type == H16_F32;
     Scalars<float> sc;
-    if (scalars_on_device) { sc.alpha = 0.f; sc.beta = 0.f; sc.alpha_dev = (const float*)alpha; sc.beta_dev = (const float*)beta; }
-    else { sc.alpha = *(const float*)alpha; sc.beta = *(const float*)beta; sc.alpha_dev = nullptr; sc.beta_dev = nullptr; }
+    set_scalars(sc, alpha, beta, scalars_on_device);
     // the workspace holds the row-major copy of a K-contiguous op(B), then the carry slots; a NULL, misaligned or smaller buffer
     // gets neither: the strided gathers and the unsplit walk, with the same bits
     void* copy = nullptr;
     const size_t need = b200spmm_csr16_workspace_bytes(k, n, nnz, sbk, sbj);
-    if (need > 0 && workspace && ((uintptr_t)workspace & 15) == 0 && workspace_bytes >= need) {
+    if (need > 0 && workspace_usable(workspace, workspace_bytes, need)) {
         const size_t cb = csr16_copy(n, sbk, sbj) ? csr16_copy_bytes(k, n) : 0;
         if (cb) copy = workspace;
         a.carry = (float*)((char*)workspace + cb);

@@ -136,13 +136,7 @@ __global__ void __launch_bounds__(RT_THREADS) spmm_csr_t_rows_kernel(const int* 
                                                                   int out_base, int* t_row) {
     const int k = (int)blockIdx.x * RT_THREADS + (int)threadIdx.x;
     if (k >= nnz) return;
-    const int x = perm ? perm[k] : k;
-    int lo = 0, hi = rows;
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (__ldg(off + mid) - base <= x) lo = mid; else hi = mid;
-    }
-    t_row[k] = lo + out_base;
+    t_row[k] = csr_row_of(off, rows, base, perm ? perm[k] : k) + out_base;
 }
 
 // tVal[k] = val[perm[k]], bit for bit (W: the value's width as an unsigned type)
@@ -153,7 +147,6 @@ __global__ void __launch_bounds__(RT_THREADS) spmm_csr_t_gather_kernel(const W* 
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-static size_t up256(size_t b) { return (b + 255) / 256 * 256; }
 static int64_t rt_ntiles(int64_t nnz) { return (nnz + RT_TILE - 1) / RT_TILE; }
 static unsigned rt_grid(int64_t n) { return (unsigned)((n + RT_THREADS - 1) / RT_THREADS); }
 
@@ -164,18 +157,18 @@ int rt_passes(int64_t nkeys) {
 }
 
 size_t rt_scratch_bytes(int64_t n) {
-    return 4 * up256((size_t)n * 4) + up256((size_t)RT_BINS * rt_ntiles(n) * 4) + up256((size_t)RT_BINS * 4);
+    return 4 * round_up_256((size_t)n * 4) + round_up_256((size_t)RT_BINS * rt_ntiles(n) * 4) + round_up_256((size_t)RT_BINS * 4);
 }
 
 RtScratch rt_scratch(char* base, int64_t n) {
-    const size_t e = up256((size_t)n * 4);
+    const size_t e = round_up_256((size_t)n * 4);
     RtScratch s;
     s.k[0] = (int*)base;
     s.k[1] = (int*)(base + e);
     s.v[0] = (int*)(base + 2 * e);
     s.v[1] = (int*)(base + 3 * e);
     s.hist = (int*)(base + 4 * e);
-    s.tot = (int*)(base + 4 * e + up256((size_t)RT_BINS * rt_ntiles(n) * 4));
+    s.tot = (int*)(base + 4 * e + round_up_256((size_t)RT_BINS * rt_ntiles(n) * 4));
     return s;
 }
 
@@ -228,15 +221,15 @@ static TLayout t_layout(int dtype, int64_t rows, int64_t cols, int64_t n, int64_
     TLayout L;
     const size_t e = (size_t)nnz * 4;
     L.t_off = 0;
-    L.t_row = up256(((size_t)cols + 1) * 4);
-    L.perm = L.t_row + up256(e);
-    L.k0 = L.perm + up256(e);
+    L.t_row = round_up_256(((size_t)cols + 1) * 4);
+    L.perm = L.t_row + round_up_256(e);
+    L.k0 = L.perm + round_up_256(e);
     L.t_val = L.k0 + rt_scratch_bytes(nnz);
-    L.ws = L.t_val + up256((size_t)nnz * elem_bytes(dtype));
+    L.ws = L.t_val + round_up_256((size_t)nnz * elem_bytes(dtype));
     // the N kernel's workspace for the cols x rows CSR matrix A^T: the row-major copy of a K-contiguous B (and the 16-bit carry slots)
     if (is16(dtype)) L.ws_bytes = b200spmm_csr16_workspace_bytes(rows, n, nnz, sbk, sbj);
     else L.ws_bytes = b200spmm_csr_workspace_bytes(dtype, rows, n, sbj == 1 ? 1 : 0);
-    L.total = L.ws + up256(L.ws_bytes);
+    L.total = L.ws + round_up_256(L.ws_bytes);
     return L;
 }
 

@@ -1,5 +1,7 @@
-// spmv_common.cuh -- device helpers shared by the CSR / COO / SELL kernels (sm_90a).
+// spmv_common.cuh -- helpers shared by the sparse kernels (sm_90a) and the host code that launches them.
 #pragma once
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -100,6 +102,13 @@ struct Scalars {
     __device__ __forceinline__ T b() const { return beta_dev ? *beta_dev : beta; }
 };
 
+// host side: device pointers kept as they are (on_device), host values read now
+template <typename T>
+void set_scalars(Scalars<T>& s, const void* alpha, const void* beta, int on_device) {
+    if (on_device) { s.alpha = T{}; s.beta = T{}; s.alpha_dev = (const T*)alpha; s.beta_dev = (const T*)beta; }
+    else { s.alpha = *(const T*)alpha; s.beta = *(const T*)beta; s.alpha_dev = nullptr; s.beta_dev = nullptr; }
+}
+
 template <typename T>
 __device__ __forceinline__ T axpby(T alpha, T sum, T beta, const T* y) {
     // beta == 0 must not read y (it may hold NaN/uninitialised memory, as cudaMalloc'ed dY does).
@@ -131,6 +140,38 @@ __device__ __forceinline__ T warp_sum(T v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
     return v;
+}
+
+// the warp's sum on every lane (xor butterfly; warp_sum leaves it on lane 0 only)
+template <typename T>
+__device__ __forceinline__ T warp_allsum(T v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+// the row (BSR: block-row) of n holding entry e < nnz: the last r with off[r] - base <= e (an empty row never holds e)
+__device__ __forceinline__ int csr_row_of(const int* off, int n, int base, int e) {
+    int lo = 0, hi = n;                      // invariant: off[lo] - base <= e < off[hi] - base (off[n] - base = nnz > e)
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (__ldg(off + mid) - base <= e) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+// a stored value widened to its accumulator type: fp16 / bf16 to fp32, fp32 and fp64 as they are
+__device__ __forceinline__ float to_acc(__half v) { return __half2float(v); }
+__device__ __forceinline__ float to_acc(__nv_bfloat16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ float to_acc(float v) { return v; }
+__device__ __forceinline__ double to_acc(double v) { return v; }
+
+// workspace sections start on 256-byte boundaries
+__host__ __device__ inline size_t round_up_256(size_t b) { return (b + 255) / 256 * 256; }
+
+// the caller's workspace can hold `need` bytes of 16-byte-aligned data
+inline bool workspace_usable(const void* ws, size_t bytes, size_t need) {
+    return ws && ((uintptr_t)ws & 15) == 0 && bytes >= need;
 }
 
 }  // namespace b200

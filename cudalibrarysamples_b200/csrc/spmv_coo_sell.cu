@@ -151,13 +151,6 @@ constexpr int COO_SEG_CHUNK = 32 * COO_SEG_STEPS;
 static_assert(COO_SEG_STEPS % COO_SEG_BATCH == 0, "steps per chunk must be a multiple of the batch");
 
 template <typename T>
-__device__ __forceinline__ T coo_warp_allsum(T v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
-template <typename T>
 __global__ void __launch_bounds__(COO_BLOCK, B200_COO_SEG_MIN_CTAS) coo_seg_kernel(const CooArgs<T> a) {
     const int lane = (int)threadIdx.x & 31;
     const long long wid = (long long)blockIdx.x * (COO_BLOCK / 32) + ((int)threadIdx.x >> 5);
@@ -203,7 +196,7 @@ __global__ void __launch_bounds__(COO_BLOCK, B200_COO_SEG_MIN_CTAS) coo_seg_kern
             const T pk = p[k]; const int rk = rr[k]; const unsigned m = mm[k];
             if (m == 0u) { acc += pk; continue; }             // the whole step lies inside one run
             const int e1 = __ffs(m) - 1, ek = 31 - __clz(m);
-            const T t1 = coo_warp_allsum(acc + (lane <= e1 ? pk : T(0)));
+            const T t1 = warp_allsum(acc + (lane <= e1 ? pk : T(0)));
             T q = (lane > e1 && lane <= ek) ? pk : T(0);
             if (m & (m - 1u)) {                               // more runs end: segmented inclusive scan
                 const unsigned below = m & ((1u << lane) - 1u);
@@ -225,8 +218,7 @@ template <typename T>
 static int launch_coo(cudaStream_t stream, int64_t rows, int64_t nnz, const void* row, const void* col, const void* val,
                       int base, const void* alpha, const void* beta, int on_device, const void* x, void* y) {
     Scalars<T> s;
-    if (on_device) { s.alpha = T(0); s.beta = T(0); s.alpha_dev = (const T*)alpha; s.beta_dev = (const T*)beta; }
-    else { s.alpha = *(const T*)alpha; s.beta = *(const T*)beta; s.alpha_dev = nullptr; s.beta_dev = nullptr; }
+    set_scalars(s, alpha, beta, on_device);
     {
         const int threads = 256;
         int64_t blocks = (rows + threads - 1) / threads;
@@ -406,8 +398,7 @@ static int launch_sell(cudaStream_t stream, int64_t rows, int64_t slice_size, co
     SellArgs<T> a;
     a.slice_off = (const int*)slice_off; a.col = (const int*)col; a.val = (const T*)val; a.x = (const T*)x; a.y = (T*)y;
     a.base = base; a.rows = (int)rows; a.slice_size = (int)slice_size;
-    if (on_device) { a.s.alpha = T(0); a.s.beta = T(0); a.s.alpha_dev = (const T*)alpha; a.s.beta_dev = (const T*)beta; }
-    else { a.s.alpha = *(const T*)alpha; a.s.beta = *(const T*)beta; a.s.alpha_dev = nullptr; a.s.beta_dev = nullptr; }
+    set_scalars(a.s, alpha, beta, on_device);
     // persistent grid of the generic kernel: SMs x resident CTAs, cached per (device, value type) under a lock
     static int grid_cache[64][2];
     static std::mutex mu;

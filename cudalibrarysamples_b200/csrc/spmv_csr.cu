@@ -107,16 +107,15 @@ struct PlanView {
 static inline int64_t csr_num_tiles(int64_t rows, int64_t nnz) {
     return (rows + nnz + CSR_TILE_ITEMS - 1) / CSR_TILE_ITEMS;
 }
-static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 static inline size_t plan_layout(int64_t num_tiles, void* ws, PlanView* v) {
     size_t n = (size_t)num_tiles + 1;
     size_t o_tiles = PLAN_HEADER_BYTES;
-    size_t o_ctl   = align_up(o_tiles + n * sizeof(int2), 256);
-    size_t o_split = align_up(o_ctl + 64, 256);
-    size_t o_head  = align_up(o_split + n * sizeof(int4), 256);
-    size_t o_tail  = align_up(o_head + n * sizeof(double), 256);
-    size_t total   = align_up(o_tail + n * sizeof(double), 256);
+    size_t o_ctl   = round_up_256(o_tiles + n * sizeof(int2));
+    size_t o_split = round_up_256(o_ctl + 64);
+    size_t o_head  = round_up_256(o_split + n * sizeof(int4));
+    size_t o_tail  = round_up_256(o_head + n * sizeof(double));
+    size_t total   = round_up_256(o_tail + n * sizeof(double));
     if (v) {
         char* b = (char*)ws;
         v->tiles = (int2*)(b + o_tiles);
@@ -513,13 +512,6 @@ constexpr int SEG_WARPS  = CSR_BLOCK / 32;
 constexpr int SEG_WSTEPS = ((CSR_SMEM_ELEMS + 31 + 31) / 32 + SEG_WARPS - 1) / SEG_WARPS;   // 32-element steps per warp, worst case
 constexpr int SEG_BATCH  = B200_SEG_BATCH;
 constexpr int SEG_BIG    = 32767;                 // "this row never ends here": sentinel behind the staged row starts
-
-template <typename T>
-__device__ __forceinline__ T warp_allsum(T v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
 
 // Number of j in [0, nr) with S[j + 1] <= lo  (S = staged row starts, non-decreasing), by the whole warp: two levels of
 // a 32-ary search instead of log2(nr) dependent probes.
@@ -1310,8 +1302,7 @@ static int launch_csr(cudaStream_t stream, int64_t rows, int64_t nnz, const void
     CsrArgs<T> a;
     a.off = (const int*)off; a.col = (const int*)col; a.val = (const T*)val;
     a.x = (const T*)x; a.y = (T*)y; a.base = base; a.rows = (int)rows; a.nnz = (int)nnz;
-    if (on_device) { a.s.alpha = T(0); a.s.beta = T(0); a.s.alpha_dev = (const T*)alpha; a.s.beta_dev = (const T*)beta; }
-    else { a.s.alpha = *(const T*)alpha; a.s.beta = *(const T*)beta; a.s.alpha_dev = nullptr; a.s.beta_dev = nullptr; }
+    set_scalars(a.s, alpha, beta, on_device);
     plan_layout(nt, ws, &a.plan);
     a.trace = nullptr;
     a.num_tiles = (unsigned)nt;

@@ -193,8 +193,7 @@ int b200spmv_csr16(void* stream, int a_type, int y_type, int64_t rows, int64_t c
     a.rows = (int)rows; a.nnz = (int)nnz; a.base = base; a.nchunks = (int)csr_walk_nchunks<MV16_CHUNK>(nnz);
     a.y_f32 = y_type == MV16_F32;
     Scalars<float> sc;
-    if (scalars_on_device) { sc.alpha = 0.f; sc.beta = 0.f; sc.alpha_dev = (const float*)alpha; sc.beta_dev = (const float*)beta; }
-    else { sc.alpha = *(const float*)alpha; sc.beta = *(const float*)beta; sc.alpha_dev = nullptr; sc.beta_dev = nullptr; }
+    set_scalars(sc, alpha, beta, scalars_on_device);
     const int lw = mv16_path(columns, values);
     const cudaStream_t st = (cudaStream_t)stream;
     if (a_type == MV16_F16) {

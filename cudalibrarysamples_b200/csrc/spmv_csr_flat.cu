@@ -105,7 +105,6 @@ struct FlatPlan {
     unsigned* bins;       // [HOT_BINS]
 };
 
-static inline size_t flat_align(size_t v) { return (v + 255) / 256 * 256; }
 static inline int64_t flat_num_ctas(int64_t nnz) { return (nnz + FLAT_CTA_NNZ - 1) / FLAT_CTA_NNZ; }
 static inline int64_t flat_num_chunks_padded(int64_t nnz) { return (nnz + FLAT_PAD_NNZ - 1) / FLAT_PAD_NNZ * (FLAT_PAD_NNZ / PLAN_CHUNK); }
 
@@ -116,19 +115,19 @@ static size_t flat_layout(int64_t rows, int64_t nnz, void* ws, FlatPlan* p) {
     const int64_t nscan_items = rows > (int64_t)ncolp ? rows : (int64_t)ncolp;
     const size_t nscan = (size_t)((nscan_items > (int64_t)nchunks ? nscan_items : (int64_t)nchunks) / SCAN_ITEMS + 2);
     size_t o = 0;
-    const size_t o_mask = o;  o = flat_align(o + nchunks * PLAN_STEPS * sizeof(unsigned));
-    const size_t o_crun = o;  o = flat_align(o + (nchunks + 1) * sizeof(int));
-    const size_t o_nzr  = o;  o = flat_align(o + ((size_t)rows + 2 + 32) * sizeof(int));   // + 32: the kernel's look-ahead window
-    const size_t o_cf   = o;  o = flat_align(o + nctas * sizeof(double));
-    const size_t o_cl   = o;  o = flat_align(o + nctas * sizeof(double));
-    const size_t o_fl   = o;  o = flat_align(o + nctas * sizeof(int));
-    const size_t o_ctl  = o;  o = flat_align(o + 64);
-    const size_t o_scr  = o;  o = flat_align(o + nscan * sizeof(int));
+    const size_t o_mask = o;  o = round_up_256(o + nchunks * PLAN_STEPS * sizeof(unsigned));
+    const size_t o_crun = o;  o = round_up_256(o + (nchunks + 1) * sizeof(int));
+    const size_t o_nzr  = o;  o = round_up_256(o + ((size_t)rows + 2 + 32) * sizeof(int));   // + 32: the kernel's look-ahead window
+    const size_t o_cf   = o;  o = round_up_256(o + nctas * sizeof(double));
+    const size_t o_cl   = o;  o = round_up_256(o + nctas * sizeof(double));
+    const size_t o_fl   = o;  o = round_up_256(o + nctas * sizeof(int));
+    const size_t o_ctl  = o;  o = round_up_256(o + 64);
+    const size_t o_scr  = o;  o = round_up_256(o + nscan * sizeof(int));
     const bool   hot = ncolp > 0;
-    const size_t o_colp = o;  o = flat_align(o + ncolp * sizeof(int));
-    const size_t o_hot  = o;  o = flat_align(o + (hot ? HOT_MAX * sizeof(int) : 0));
-    const size_t o_xh   = o;  o = flat_align(o + (hot ? HOT_BYTES : 0));
-    const size_t o_bins = o;  o = flat_align(o + (hot ? HOT_BINS * sizeof(unsigned) : 0));
+    const size_t o_colp = o;  o = round_up_256(o + ncolp * sizeof(int));
+    const size_t o_hot  = o;  o = round_up_256(o + (hot ? HOT_MAX * sizeof(int) : 0));
+    const size_t o_xh   = o;  o = round_up_256(o + (hot ? HOT_BYTES : 0));
+    const size_t o_bins = o;  o = round_up_256(o + (hot ? HOT_BINS * sizeof(unsigned) : 0));
     if (p) {
         char* b = (char*)ws;
         p->endmask = (unsigned*)(b + o_mask); p->chunk_run = (int*)(b + o_crun); p->nzrow = (int*)(b + o_nzr);
@@ -174,8 +173,7 @@ __global__ void __launch_bounds__(256) scan_block_sums_kernel(V value, int64_t n
         const int64_t i = i0 + k;
         s += i < n ? value(i) : 0;
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    s = warp_allsum(s);
     if ((threadIdx.x & 31) == 0) sw[threadIdx.x >> 5] = s;
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -263,8 +261,7 @@ __global__ void flat_finish_kernel(FlatPlan p, int64_t rows, int64_t nchunks, in
     int quiet = 0;
     for (int64_t w = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; w < nwords; w += (int64_t)gridDim.x * blockDim.x)
         quiet += p.endmask[w] == 0u;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) quiet += __shfl_xor_sync(0xffffffffu, quiet, o);
+    quiet = warp_allsum(quiet);
     if ((threadIdx.x & 31) == 0 && quiet) atomicAdd(p.ctl + 1, quiet);
 }
 
@@ -348,13 +345,6 @@ struct FlatArgs {
     Scalars<T> s;
     FlatPlan   plan;
 };
-
-template <typename T>
-__device__ __forceinline__ T flat_allsum(T v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
 
 // y[r] = alpha * v + beta * y[r]; beta == 0 never reads y (predicated load, no branch)
 template <typename T>
@@ -441,7 +431,7 @@ __global__ void __launch_bounds__(FLAT_BLOCK, B200_FLAT_MIN_CTAS) csr_flat_kerne
 #else
                 if (is_end) row = __ldg(a.plan.nzrow + run + __popc(m & ((1u << lane) - 1u)) + 1);   // (run + k)-th non-empty row
 #endif
-                const T t1 = flat_allsum(acc + (lane <= e1 ? pk : T(0)));
+                const T t1 = warp_allsum(acc + (lane <= e1 ? pk : T(0)));
                 T q = (lane > e1 && lane <= ek) ? pk : T(0);
                 if (m & (m - 1u)) {                        // more rows end: segmented inclusive scan
                     const unsigned below = m & ((1u << lane) - 1u);
@@ -468,7 +458,7 @@ __global__ void __launch_bounds__(FLAT_BLOCK, B200_FLAT_MIN_CTAS) csr_flat_kerne
         // non-zeros behind the chunk's last row end belong to a row that continues in the next chunk
         const int  el = n1 - 1 - n0;                       // the chunk's last live element
         const unsigned ml = __shfl_sync(0xffffffffu, mreg, el >> 5);
-        if (!((ml >> (el & 31)) & 1u)) last = flat_allsum(acc);
+        if (!((ml >> (el & 31)) & 1u)) last = warp_allsum(acc);
     }
     // The warp that deposits its partials LAST stitches the CTA (fixed warp order -> bit-reproducible); the others are gone.
     int arrived = 0;
@@ -565,8 +555,7 @@ static int launch_flat(cudaStream_t stream, int64_t rows, int64_t nnz, const voi
     FlatArgs<T> a;
     a.off = (const int*)off; a.col = (const int*)col; a.val = (const T*)val; a.x = (const T*)x; a.y = (T*)y;
     a.base = base; a.rows = (int)rows; a.nnz = (int)nnz;
-    if (on_device) { a.s.alpha = T(0); a.s.beta = T(0); a.s.alpha_dev = (const T*)alpha; a.s.beta_dev = (const T*)beta; }
-    else { a.s.alpha = *(const T*)alpha; a.s.beta = *(const T*)beta; a.s.alpha_dev = nullptr; a.s.beta_dev = nullptr; }
+    set_scalars(a.s, alpha, beta, on_device);
     flat_layout(rows, nnz, ws, &a.plan);
     a.xh = (const T*)a.plan.xh;
     stats().last_csr_kernel = sizeof(T) == 8 ? "b200::csr_flat_kernel<double>" : "b200::csr_flat_kernel<float>";

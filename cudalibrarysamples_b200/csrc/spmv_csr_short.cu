@@ -107,8 +107,7 @@ csr_short_kernel(const ShortArgs<T> a) {
         // deterministic three-level sum: lanes (butterfly), warps of the CTA (in warp order), CTAs (in CTA order, by the CTA
         // that arrives last) -- same scheme as csrc/cg_fused.cu
         __shared__ double swarp[SHORT_WARPS];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
+        dsum = warp_allsum(dsum);
         if (lane == 0) swarp[warp] = dsum;
         __syncthreads();
         if (threadIdx.x == 0) {
@@ -147,8 +146,7 @@ static int launch_short(cudaStream_t stream, int64_t rows, const void* off, cons
     a.w = (const T*)w; a.dot_out = dot_out; a.dot_ws = (double*)dot_ws;
     a.off = (const int*)off; a.col = (const int*)col; a.val = (const T*)val; a.x = (const T*)x; a.y = (T*)y;
     a.base = base; a.rows = (int)rows;
-    if (on_device) { a.s.alpha = T(0); a.s.beta = T(0); a.s.alpha_dev = (const T*)alpha; a.s.beta_dev = (const T*)beta; }
-    else { a.s.alpha = *(const T*)alpha; a.s.beta = *(const T*)beta; a.s.alpha_dev = nullptr; a.s.beta_dev = nullptr; }
+    set_scalars(a.s, alpha, beta, on_device);
     stats().last_csr_kernel = sizeof(T) == 8 ? "b200::csr_short_kernel<double>" : "b200::csr_short_kernel<float>";
     const int64_t nblocks = (rows + 31) / 32;
     int64_t ctas = (nblocks + SHORT_WARPS - 1) / SHORT_WARPS;

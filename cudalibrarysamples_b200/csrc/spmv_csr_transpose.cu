@@ -48,13 +48,7 @@ __global__ void __launch_bounds__(TR_BLOCK) csr_transpose_kernel(const TrArgs<T>
     if (c0 >= a.nnz) return;                                       // warp-uniform
     const int n0 = (int)c0, n1 = min(n0 + TR_CHUNK, a.nnz);
     const T alpha = a.s.a();
-    // row of non-zero n0: the last r with off[r] - base <= n0 (empty rows in front of it are skipped by the upper bound)
-    int lo = 0, hi = a.rows;                                       // invariant: off[lo] - base <= n0 < off[hi] - base (off[rows] = nnz > n0)
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (__ldg(a.off + mid) - a.base <= n0) lo = mid; else hi = mid;
-    }
-    int r = lo;
+    int r = csr_row_of(a.off, a.rows, a.base, n0);
     int rend = __ldg(a.off + r + 1) - a.base;                      // first non-zero behind my current row
     int cc[TR_STEPS];
     T   vv[TR_STEPS];
@@ -81,8 +75,7 @@ static int launch_transpose(cudaStream_t stream, int64_t rows, int64_t cols, int
     TrArgs<T> a;
     a.off = (const int*)off; a.col = (const int*)col; a.val = (const T*)val; a.x = (const T*)x; a.y = (T*)y;
     a.base = base; a.rows = (int)rows; a.cols = (int)cols; a.nnz = (int)nnz;
-    if (on_device) { a.s.alpha = T(0); a.s.beta = T(0); a.s.alpha_dev = (const T*)alpha; a.s.beta_dev = (const T*)beta; }
-    else { a.s.alpha = *(const T*)alpha; a.s.beta = *(const T*)beta; a.s.alpha_dev = nullptr; a.s.beta_dev = nullptr; }
+    set_scalars(a.s, alpha, beta, on_device);
     stats().last_csr_kernel = sizeof(T) == 8 ? "b200::csr_transpose_kernel<double>" : "b200::csr_transpose_kernel<float>";
     if (cols > 0 && (on_device || *(const T*)beta != T(1))) {
         int64_t blocks = (cols + 255) / 256;

@@ -165,7 +165,7 @@ __global__ void __launch_bounds__(256) spmv_csrz_transpose_kernel(const SpmvCsrZ
     if (c0 >= a.nnz) return;                                       // warp-uniform
     const int n0 = (int)c0, n1 = min(n0 + MVZ_TR_CHUNK, a.nnz);
     const double2 alpha = sc.a();
-    int r = csr_last_row(a, n0);                                   // the row of entry n0
+    int r = csr_row_of(a.off, a.rows, a.base, n0);                 // the row of entry n0
     int rend = csr_off(a, r + 1);
     constexpr int STEPS = MVZ_TR_CHUNK / 32;
     int cc[STEPS];
@@ -228,12 +228,7 @@ int b200spmv_csr_z(void* stream, int op, int64_t rows, int64_t cols, int64_t nnz
     a.rows = (int)rows; a.cols = (int)cols; a.nnz = (int)nnz; a.base = base; a.nchunks = (int)csr_walk_nchunks<MVZ_CHUNK>(nnz);
     a.conj = op == 2;
     Scalars<double2> sc;
-    if (scalars_on_device) {
-        sc.alpha = sc.beta = make_double2(0.0, 0.0);
-        sc.alpha_dev = (const double2*)alpha; sc.beta_dev = (const double2*)beta;
-    } else {
-        sc.alpha = *(const double2*)alpha; sc.beta = *(const double2*)beta; sc.alpha_dev = nullptr; sc.beta_dev = nullptr;
-    }
+    set_scalars(sc, alpha, beta, scalars_on_device);
     const cudaStream_t st = (cudaStream_t)stream;
     if (tr) {
         stats().last_csr_kernel = "b200::spmv_csrz_transpose_kernel";

@@ -26,12 +26,6 @@
 namespace b200 {
 
 // ------------------------------------------------------------------------------------------------ host side
-template <typename XT>
-static void set_scalars(Scalars<XT>& s, const void* alpha, const void* beta, int on_device) {
-    if (on_device) { s.alpha = XT(0); s.beta = XT(0); s.alpha_dev = (const XT*)alpha; s.beta_dev = (const XT*)beta; }
-    else { s.alpha = *(const XT*)alpha; s.beta = *(const XT*)beta; s.alpha_dev = nullptr; s.beta_dev = nullptr; }
-}
-
 static unsigned grid_for(long long threads) {
     long long ctas = (threads + GEN_BLOCK - 1) / GEN_BLOCK;
     if (ctas < 1) ctas = 1;

@@ -28,13 +28,13 @@ constexpr int kThreads = 256;          // solve kernel: 8 warps (rows in flight)
 static void layout(int64_t rows, int64_t nnz, int transpose, size_t* o) {
     size_t p = 0;
     o[B200SPSM_STATE] = p;   p += 256;
-    o[B200SPSM_FLAGS] = p;   p += align256(4 * (size_t)rows);
-    o[B200SPSM_T_OFF] = p;   p += align256(4 * ((size_t)rows + 1));
-    o[B200SPSM_DIAG] = p;    p += align256(4 * (size_t)rows);
-    o[B200SPSM_T_COL] = p;   p += align256(4 * (size_t)nnz);
-    o[B200SPSM_T_VIDX] = p;  p += align256(4 * (size_t)nnz);
-    o[B200SPSM_ORDER] = p;   p += align256(4 * (size_t)rows);
-    o[B200SPSM_SCRATCH] = p; p += align256(4 * (size_t)rows) + (transpose ? 2 * align256(4 * (size_t)nnz) : 0);
+    o[B200SPSM_FLAGS] = p;   p += round_up_256(4 * (size_t)rows);
+    o[B200SPSM_T_OFF] = p;   p += round_up_256(4 * ((size_t)rows + 1));
+    o[B200SPSM_DIAG] = p;    p += round_up_256(4 * (size_t)rows);
+    o[B200SPSM_T_COL] = p;   p += round_up_256(4 * (size_t)nnz);
+    o[B200SPSM_T_VIDX] = p;  p += round_up_256(4 * (size_t)nnz);
+    o[B200SPSM_ORDER] = p;   p += round_up_256(4 * (size_t)rows);
+    o[B200SPSM_SCRATCH] = p; p += round_up_256(4 * (size_t)rows) + (transpose ? 2 * round_up_256(4 * (size_t)nnz) : 0);
     o[B200SPSM_TOTAL] = p;
 }
 

@@ -20,12 +20,12 @@ constexpr int      kThreads = 256;                        // solve kernel: 8 war
 static void layout(int64_t rows, int64_t nnz, int transpose, size_t* o) {
     size_t p = 0;
     o[B200SPSV_STATE] = p;   p += 256;
-    o[B200SPSV_FLAGS] = p;   p += align256(4 * (size_t)rows);
-    o[B200SPSV_T_OFF] = p;   p += align256(4 * ((size_t)rows + 1));
-    o[B200SPSV_DIAG] = p;    p += align256(4 * (size_t)rows);
-    o[B200SPSV_T_COL] = p;   p += align256(4 * (size_t)nnz);
-    o[B200SPSV_T_VIDX] = p;  p += align256(4 * (size_t)nnz);
-    o[B200SPSV_SCRATCH] = p; p += align256(4 * (size_t)rows) + (transpose ? 2 * align256(4 * (size_t)nnz) : 0);
+    o[B200SPSV_FLAGS] = p;   p += round_up_256(4 * (size_t)rows);
+    o[B200SPSV_T_OFF] = p;   p += round_up_256(4 * ((size_t)rows + 1));
+    o[B200SPSV_DIAG] = p;    p += round_up_256(4 * (size_t)rows);
+    o[B200SPSV_T_COL] = p;   p += round_up_256(4 * (size_t)nnz);
+    o[B200SPSV_T_VIDX] = p;  p += round_up_256(4 * (size_t)nnz);
+    o[B200SPSV_SCRATCH] = p; p += round_up_256(4 * (size_t)rows) + (transpose ? 2 * round_up_256(4 * (size_t)nnz) : 0);
     o[B200SPSV_TOTAL] = p;
 }
 

@@ -10,6 +10,8 @@
 #include <algorithm>
 #include <cstdint>
 
+#include "spmv_common.cuh"
+
 namespace b200spsv {
 
 constexpr int      kAnalysisThreads = 256;
@@ -17,7 +19,7 @@ constexpr int      kScanThreads = 1024;
 constexpr uint64_t kSpinBudgetNs = 4000000000ull;         // 4 s per wait: far beyond any legitimate wait, well inside a watchdog
 enum { ST_EPOCH = 0, ST_CLAIM = 1, ST_ERROR = 2, ST_MISSING = 3 };
 
-static inline size_t align256(size_t b) { return (b + 255) / 256 * 256; }
+using b200::round_up_256;
 
 // ------------------------------------------------------------------------------------------------ analysis
 // Per row r of A: the first stored diagonal (NON_UNIT), and the number of selected off-diagonal entries -- of row r of
@@ -129,8 +131,8 @@ static cudaError_t build_plan(cudaStream_t s, int64_t rows, int64_t nnz, const i
         if (!transpose) {
             fill_rows_kernel<<<blocks, kAnalysisThreads, 0, s>>>(n, off, col, base, lower, t_off, t_col, t_vidx);
         } else {
-            int* tmp_row = (int*)(scratch + align256(4 * (size_t)rows));
-            int* tmp_k = (int*)((char*)tmp_row + align256(4 * (size_t)nnz));
+            int* tmp_row = (int*)(scratch + round_up_256(4 * (size_t)rows));
+            int* tmp_k = (int*)((char*)tmp_row + round_up_256(4 * (size_t)nnz));
             err = cudaMemsetAsync(cnt, 0, 4 * (size_t)rows, s);                                // counts -> cursors
             if (err != cudaSuccess) return err;
             scatter_cols_kernel<<<blocks, kAnalysisThreads, 0, s>>>(n, off, col, base, lower, t_off, cnt, tmp_row, tmp_k);
