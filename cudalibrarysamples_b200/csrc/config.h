@@ -23,6 +23,9 @@ struct Config {
     int zcsr        = 0;    // B200SPMV_ZCSR = auto|on: cusparseSpMV on a double-complex CSR A.  auto (0, default): b200spmv_csr_z
                             //   only in the classes measured at least at parity (none today, DESIGN.md 3.21); on (1): every call
                             //   in b200spmv_csr_z's class
+    int dense       = 0;    // B200SPMV_DENSE = auto|on: cusparseSparseToDense / cusparseDenseToSparse_convert.  auto (0, default):
+                            //   the native kernels only in the classes measured at least at parity (DESIGN.md 3.24); on (1): every
+                            //   call b200dense_route admits, so the shim's native path can be exercised before a measurement routes it
 };
 
 Config& config();

@@ -127,6 +127,12 @@ def shim(build_if_missing: bool = False) -> C.CDLL:
         lib.b200csr2coo.argtypes = [vp, vp, i64, i64, vp, C.c_int32]
         lib.b200identity_permutation.argtypes = [vp, i64, vp]
         lib.b200conv_route.argtypes = [C.c_int, i64, i64, i64, C.c_int, C.c_int, vp]
+        lib.b200csr2dense.argtypes = [vp, C.c_int, i64, i64, i64, vp, vp, vp, C.c_int, C.c_int32, vp, i64, C.c_int]
+        lib.b200coo2dense.argtypes = [vp, i64, i64, i64, vp, vp, vp, C.c_int, C.c_int32, vp, i64, C.c_int]
+        lib.b200bell2dense.argtypes = [vp, i64, i64, i64, i64, vp, vp, C.c_int, C.c_int32, vp, i64, C.c_int]
+        lib.b200dense2csr.argtypes = [vp, C.c_int, i64, i64, i64, vp, i64, C.c_int, C.c_int, vp, vp, vp, C.c_int32]
+        lib.b200dense2bell.argtypes = [vp, i64, i64, i64, i64, vp, i64, C.c_int, C.c_int, vp, vp, C.c_int32]
+        lib.b200dense_route.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, i64, i64, i64, C.c_int, C.c_int, i64]
         lib.b200spmv_csr16.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, vp, vp, C.c_size_t]
         lib.b200spmv_csr16_workspace_bytes.argtypes = [i64, i64]
         lib.b200spmv_csr16_workspace_bytes.restype = C.c_size_t

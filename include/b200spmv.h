@@ -400,6 +400,43 @@ B200SPMV_EXPORT int b200coo2csr(void* stream, const void* coo_row_ind, int64_t n
 B200SPMV_EXPORT int b200csr2coo(void* stream, const void* csr_row_ptr, int64_t nnz, int64_t m, void* coo_row_ind, int32_t base);
 B200SPMV_EXPORT int b200identity_permutation(void* stream, int64_t n, void* p);
 
+/* Sparse <-> dense conversion (dense_convert.cu), int32 indices, base 0 or 1.  The dense operand is rows x cols in order
+ * 1 (CUSPARSE_ORDER_COL) or 2 (CUSPARSE_ORDER_ROW), the cusparseOrder_t values, with ld >= max(1, its contiguous dimension).  Values
+ * move bit for bit by width (2, 4, 8 or 16 bytes).  No allocation, no host synchronisation, no floating-point atomics:
+ * graph-capturable, and every result a pure function of the input.  Each returns -1 with nothing launched on bad sizes, base,
+ * width, value type, order or ld, or on a NULL or misaligned pointer the call needs, else the CUDA launch status.
+ *
+ * Sparse -> dense (cusparseSparseToDense): every element of the m x n window of dense is written, zero where A has no entry;
+ * nothing else is (not the ld padding).  Entries whose index lies outside the matrix are skipped.
+ *   b200csr2dense   A m x n CSR (off[m + 1], ind = columns) or, with csc nonzero, CSC (off[n + 1], ind = rows), nnz entries
+ *                   (ind / val may be NULL when nnz = 0); offsets are clamped to [0, nnz].  Duplicate entries within a row (CSC: a
+ *                   column): the last in storage order wins.
+ *   b200coo2dense   A as nnz (row, col) pairs; duplicate pairs leave one of their values.
+ *   b200bell2dense  A Blocked-ELL: bs x bs blocks, colind[(m / bs) x (ell_cols / bs)] block columns (-1 or any index outside
+ *                   the matrix: an empty slot, never read), val[m x ell_cols] row-major.  A block column named twice in a block
+ *                   row: the last slot wins. */
+B200SPMV_EXPORT int b200csr2dense(void* stream, int csc, int64_t m, int64_t n, int64_t nnz, const void* off, const void* ind, const void* val,
+                                  int value_bytes, int32_t base, void* dense, int64_t ld, int order);
+B200SPMV_EXPORT int b200coo2dense(void* stream, int64_t m, int64_t n, int64_t nnz, const void* rows, const void* cols, const void* val,
+                                  int value_bytes, int32_t base, void* dense, int64_t ld, int order);
+B200SPMV_EXPORT int b200bell2dense(void* stream, int64_t m, int64_t n, int64_t bs, int64_t ell_cols, const void* colind, const void* val,
+                                   int value_bytes, int32_t base, void* dense, int64_t ld, int order);
+/* Dense -> sparse (cusparseDenseToSparse_convert), after the closed library's analysis has written the offsets:
+ *   b200dense2csr   CSR (or CSC, csc nonzero) columns (rows) and values of every non-zero of dense, in ascending order, line i
+ *                   at off[i] - base onwards and never at or past off[i + 1] - base (both clamped to [0, nnz]): a line with more non-zeros than its range
+ *                   keeps the first ones, one with fewer leaves the rest unwritten.  value_type: a cudaDataType among 16F, 16BF,
+ *                   32F, 64F, C_32F and C_64F (complex fp16 / bf16 are refused: their predicate was not pinned); non-zero is
+ *                   "v != 0" per part as the closed analysis counts it: denormals, Inf and NaN included, +-0 excluded -- and a
+ *                   16-bit value whose magnitude bits exceed 0x7C00 excluded (that analysis reads fp16 and bf16 bits alike as
+ *                   fp16: fp16 NaN; bf16 from about 2.7e36 up).
+ *   b200dense2bell  val[m x ell_cols] of the Blocked-ELL matrix whose colind is given: each slot gets the dense bs x bs block it
+ *                   names (zero past the matrix' edge); a slot of -1 (any index outside the matrix) gets zeros, as the closed
+ *                   convert writes them. */
+B200SPMV_EXPORT int b200dense2csr(void* stream, int csc, int64_t m, int64_t n, int64_t nnz, const void* dense, int64_t ld, int order,
+                                  int value_type, const void* off, void* ind, void* val, int32_t base);
+B200SPMV_EXPORT int b200dense2bell(void* stream, int64_t m, int64_t n, int64_t bs, int64_t ell_cols, const void* dense, int64_t ld,
+                                   int order, int value_bytes, const void* colind, void* val, int32_t base);
+
 /* The BLAS-1 part of a CG iteration, fused, all scalars in DEVICE memory (no host synchronisation, CUDA-graph capturable).
  * Replaces the cublasDdot / cublasDaxpy / cublasDnrm2 / cublasDscal calls between two cusparseSpMV calls of gpu_CG
  * (cuSPARSE/cg/cg_example.c:226-286).  fp64; vectors 16-byte aligned; `workspace` = b200cg_workspace_bytes() bytes, zeroed
@@ -566,6 +603,18 @@ B200SPMV_EXPORT int b200spmv_plan_trusted(const void* matA, void* buffer, int ki
 #define B200CONV_CSR2COO 4
 #define B200CONV_IDENTITY 5
 B200SPMV_EXPORT int b200conv_route(int op, int64_t m, int64_t n, int64_t nnz, int arg, int alg, const void* buffer);
+/* Where the shim sends cusparseSparseToDense (direction B200DENSE_S2D) or cusparseDenseToSparse_convert (B200DENSE_D2S): 1 = the
+ * native entry point above, 0 = the closed library.  format: cusparseFormat_t of the sparse side; order: cusparseOrder_t of the
+ * dense side; vtype: cudaDataType; off_type / col_type: cusparseIndexType_t; batch: the larger strided-batch count of the two
+ * descriptors; alg: the call's algorithm; bs: the Blocked-ELL block size (ignored for other formats).  Forwarded:
+ * B200SPMV_FORWARD=1, 64-bit indices, a base other than 0 / 1, integer, complex fp16 / bf16 or unknown value types for dense ->
+ * CSR / CSC, dense -> COO, strided batches, an alg other than DEFAULT, and every class not measured at least at parity with the
+ * closed library (DESIGN.md 3.24; today only dense -> Blocked-ELL, row-major, bs 16, fp16 / fp32, 8192 to 16384 rows and columns
+ * is native).  B200SPMV_DENSE=on makes every call this admits native.  Host logic only. */
+#define B200DENSE_S2D 0
+#define B200DENSE_D2S 1
+B200SPMV_EXPORT int b200dense_route(int direction, int format, int order, int vtype, int off_type, int col_type, int base, int64_t rows,
+                                    int64_t cols, int64_t nnz, int batch, int alg, int64_t bs);
 /* ---------------------------------------------------------------------------------------------- *
  * Sparse triangular solve with many right-hand sides (cusparseSpSM; cuSPARSE/spsm_csr):           *
  *   C = alpha op(T)^-1 op(B), T the selected triangle of the rows x rows CSR matrix A (int32       *
@@ -741,6 +790,12 @@ B200SPMV_EXPORT cusparseStatus_t cusparseXcoosortByColumn(cusparseHandle_t, int,
 B200SPMV_EXPORT cusparseStatus_t cusparseXcoo2csr(cusparseHandle_t, const int*, int, int, int*, cusparseIndexBase_t);
 B200SPMV_EXPORT cusparseStatus_t cusparseXcsr2coo(cusparseHandle_t, const int*, int, int, int*, cusparseIndexBase_t);
 B200SPMV_EXPORT cusparseStatus_t cusparseCreateIdentityPermutation(cusparseHandle_t, int, int*);
+/* cusparse.h:5622-5663 -- sparse2dense_csr_example.c, dense2sparse_csr_example.c, dense2sparse_blockedell_example.c.  The
+ * bufferSize calls and cusparseDenseToSparse_analysis stay the closed library's. */
+B200SPMV_EXPORT cusparseStatus_t cusparseSparseToDense(cusparseHandle_t, cusparseConstSpMatDescr_t, cusparseDnMatDescr_t,
+                                                       cusparseSparseToDenseAlg_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseDenseToSparse_convert(cusparseHandle_t, cusparseConstDnMatDescr_t, cusparseSpMatDescr_t,
+                                                               cusparseDenseToSparseAlg_t, void*);
 #ifdef __cplusplus
 }
 #endif
