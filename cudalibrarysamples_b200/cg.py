@@ -78,15 +78,13 @@ class FusedCgSolver:
     iterations are captured in a CUDA graph and replayed (graph_capture_example.c:118-135 pattern)."""
 
     def __init__(self, sh: ShardedCsr, b_shard: torch.Tensor, use_graph: bool | None = None):
-        import ctypes as C
         import os
         from . import lib as _lib
-        self.C, self.L = C, _lib.shim()
-        self.L.b200cg_workspace_bytes.restype = C.c_size_t
+        self.L = _lib.shim()
         self.sh, self.b = sh, b_shard
         self.n = int(b_shard.numel())
         dev = b_shard.device
-        self.ws = torch.zeros(int(self.L.b200cg_workspace_bytes()), dtype=torch.uint8, device=dev)
+        self.ws = torch.zeros(self.L.b200cg_workspace_bytes(), dtype=torch.uint8, device=dev)
         self.scal = torch.zeros(8, dtype=torch.float64, device=dev)        # [0], [1]: delta of even / odd iterations, [2]: t.p
         self.use_graph = (sh.world == 1 and os.environ.get("B200CG_GRAPH", "1") != "0") if use_graph is None else use_graph
         self.graph_error = None
@@ -96,23 +94,20 @@ class FusedCgSolver:
         self.fuse_dot = os.environ.get("B200CG_FUSE_DOT", "0") == "1" and hasattr(sh, "can_fuse_dot") and sh.can_fuse_dot()
 
     def _stream(self):
-        return self.C.c_void_p(torch.cuda.current_stream().cuda_stream)
+        return torch.cuda.current_stream().cuda_stream
 
     def _check(self, rc, what):
         if rc != 0:
             raise RuntimeError(f"{what} failed with code {rc}")
 
-    def _p(self, t):
-        return self.C.c_void_p(t.data_ptr())
-
     def _dot(self, a, b, out):
-        self._check(self.L.b200cg_dot(self._stream(), self.C.c_int64(self.n), self._p(a), self._p(b), self._p(out), self._p(self.ws)), "b200cg_dot")
+        self._check(self.L.b200cg_dot(self._stream(), self.n, a.data_ptr(), b.data_ptr(), out.data_ptr(), self.ws.data_ptr()), "b200cg_dot")
         if self.sh.world > 1:
             dist.all_reduce(out, group=self.sh.group)
 
     def _iteration(self, x, r, p, t, cur):
         """one CG iteration; delta_k lives in scal[cur], delta_{k+1} goes to scal[1 - cur]"""
-        C, s = self.C, self.scal
+        s = self.scal
         if self.fuse_dot:
             self.sh.spmv_dot(p, t, s[2:3])                                   # T = A * P and denom = T . P in one pass (:220-227)
             if self.sh.world > 1:
@@ -122,12 +117,12 @@ class FusedCgSolver:
             self._dot(t, p, s[2:3])                                          # denom = T . P  (:227)
         nxt = 1 - cur
         # 8 vector passes after the dot's 2: R -= aT with delta' = R.R, then X += aP and P = R + (delta'/delta) P in one pass (P read once)
-        self._check(self.L.b200cg_update_r(self._stream(), C.c_int64(self.n), self._p(r), self._p(t), self._p(s[cur:cur + 1]), self._p(s[2:3]),
-                                           self._p(s[nxt:nxt + 1]), self._p(self.ws)), "b200cg_update_r")       # (:241-247)
+        self._check(self.L.b200cg_update_r(self._stream(), self.n, r.data_ptr(), t.data_ptr(), s[cur:cur + 1].data_ptr(), s[2:3].data_ptr(),
+                                           s[nxt:nxt + 1].data_ptr(), self.ws.data_ptr()), "b200cg_update_r")       # (:241-247)
         if self.sh.world > 1:
             dist.all_reduce(s[nxt:nxt + 1], group=self.sh.group)
-        self._check(self.L.b200cg_update_xp(self._stream(), C.c_int64(self.n), self._p(x), self._p(p), self._p(r), self._p(s[cur:cur + 1]),
-                                            self._p(s[2:3]), self._p(s[nxt:nxt + 1])), "b200cg_update_xp")       # (:236-239, :280-286)
+        self._check(self.L.b200cg_update_xp(self._stream(), self.n, x.data_ptr(), p.data_ptr(), r.data_ptr(), s[cur:cur + 1].data_ptr(),
+                                            s[2:3].data_ptr(), s[nxt:nxt + 1].data_ptr()), "b200cg_update_xp")       # (:236-239, :280-286)
 
     def run(self, iters: int):
         x = torch.zeros_like(self.b)

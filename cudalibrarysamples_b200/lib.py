@@ -1,13 +1,61 @@
 """ctypes loader for libb200spmv.so (the product) and the real libcusparse.so.12 (handle management + GPU oracle).
 
 The product path fails LOUDLY when the CUDA extension is missing: there is no CPU or library fallback here.
+
+Every b200* entry point of our three libraries gets its argtypes / restype from the prototype in include/ (load()), so a
+caller passes plain ints, data_ptr()s, None and floats, and ctypes converts them to exactly the C types the header names.
 """
 from __future__ import annotations
 
 import ctypes as C
+import functools
 import os
+import re
 
 from . import build as _build
+
+INCLUDE_DIR = os.path.join(os.path.dirname(_build.PKG_DIR), "include")
+_C_TYPES = {"int": C.c_int, "int32_t": C.c_int32, "int64_t": C.c_int64, "size_t": C.c_size_t, "uint64_t": C.c_uint64,
+            "double": C.c_double, "void": None}
+_PROTOTYPE = re.compile(r"\bB200\w*_EXPORT\s+([\w\s\*]+?)\s*\b(\w+)\s*\(([^)]*)\)\s*;")
+
+
+def _c_type(decl: str, what: str):
+    """The ctypes type of `decl`, a return type or a parameter with or without its name."""
+    words = decl.replace("*", " * ").split()
+    if "*" in words:
+        return C.c_char_p if words[0:2] == ["const", "char"] else C.c_void_p
+    words = [w for w in words if w != "const"]
+    if not words or words[0] not in _C_TYPES or len(words) > 2:
+        raise ValueError(f"{what}: no ctypes type for {decl!r}")
+    return _C_TYPES[words[0]]
+
+
+@functools.lru_cache(maxsize=None)
+def prototypes(header: str) -> tuple:
+    """(return type, name, parameters) of every function include/<header> tags B200*_EXPORT, cusparse* ones included."""
+    with open(os.path.join(INCLUDE_DIR, header)) as f:
+        return tuple(_PROTOTYPE.findall(re.sub(r"/\*.*?\*/|//[^\n]*", " ", f.read(), flags=re.S)))
+
+
+def signatures(header: str) -> dict:
+    """{name: (restype, argtypes)} of every b200* prototype in include/<header>."""
+    sigs = {}
+    for ret, name, params in prototypes(header):
+        if name.startswith("b200"):
+            params = [p.strip() for p in params.split(",")]
+            sigs[name] = (_c_type(ret, name), [] if params in ([""], ["void"]) else [_c_type(p, name) for p in params])
+    return sigs
+
+
+def load(path: str, header: str = "b200spmv.h", mode: int = C.RTLD_LOCAL) -> C.CDLL:
+    """CDLL(path) with every b200* function of include/<header> declared; a declared name the library lacks raises."""
+    lib = C.CDLL(path, mode=mode)
+    for name, (restype, argtypes) in signatures(header).items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
+    return lib
+
 
 def _bundled_with_torch() -> str:
     """torch's own libcusparse.so.12 (nvidia-cusparse-cu12 wheel).  Inside a Python process that imported torch, the
@@ -21,12 +69,11 @@ def _bundled_with_torch() -> str:
         return ""
 
 
-REAL_CUSPARSE_CANDIDATES = (
-    os.environ.get("B200SPMV_CUSPARSE", ""),
-    _bundled_with_torch(),
-    "/usr/local/cuda/lib64/libcusparse.so.12",
-    "libcusparse.so.12",
-)
+def _real_cusparse_candidates() -> tuple:
+    # looked up on first use, so that importing this module (as load()'s subprocess callers do) does not import torch
+    return (os.environ.get("B200SPMV_CUSPARSE", ""), _bundled_with_torch(), "/usr/local/cuda/lib64/libcusparse.so.12",
+            "libcusparse.so.12")
+
 
 _shim = None
 _spsv = None
@@ -40,7 +87,7 @@ def real() -> C.CDLL:
     global _real, _real_path
     if _real is None:
         errors = []
-        for p in REAL_CUSPARSE_CANDIDATES:
+        for p in _real_cusparse_candidates():
             if not p or ("/" in p and not os.path.exists(p)):
                 continue
             try:
@@ -73,84 +120,7 @@ def shim(build_if_missing: bool = False) -> C.CDLL:
                 raise RuntimeError(
                     f"{path} is missing: the CUDA extension was not built. Run `python -c 'import __graft_entry__ as g; "
                     "g.build()'` (nvcc, sm_90a). There is no CPU fallback.")
-        lib = C.CDLL(path, mode=C.RTLD_LOCAL)
-        lib.b200spmv_csr_workspace_bytes.restype = C.c_size_t
-        lib.b200spmv_coo_workspace_bytes.restype = C.c_size_t
-        lib.b200spmv_sell_workspace_bytes.restype = C.c_size_t
-        lib.b200spmv_csr_plan_tiles_offset.restype = C.c_size_t
-        lib.b200spmv_csr_plan_ctl_offset.restype = C.c_size_t
-        lib.b200spmv_csr_plan_split_offset.restype = C.c_size_t
-        lib.b200spmv_csr_num_tiles.restype = C.c_int64
-        lib.b200spmv_version.restype = C.c_char_p
-        lib.b200sddmm_csr_workspace_bytes.restype = C.c_size_t
-        i64, vp = C.c_int64, C.c_void_p
-        lib.b200spmm_bell.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, i64, i64, vp, vp, C.c_int32, vp, vp, C.c_int, vp, i64, C.c_int,
-                                      vp, i64, C.c_int]
-        lib.b200spmm_bell_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
-        lib.b200spmm_coo.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, i64, C.c_int,
-                                     vp, i64, C.c_int, C.c_int, i64, i64, i64, vp, C.c_size_t]
-        lib.b200spmm_coo_workspace_bytes.argtypes = [C.c_int, C.c_int, i64, i64, i64, i64, C.c_int, C.c_int, i64]
-        lib.b200spmm_coo_workspace_bytes.restype = C.c_size_t
-        lib.b200spmm_coo_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
-        lib.b200sddmm_bsr.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, i64, i64, vp, vp, vp, C.c_int32, C.c_int, vp, vp, C.c_int,
-                                      vp, i64, i64, vp, i64, i64, C.c_int, i64, i64, i64, i64, i64]
-        lib.b200sddmm_bsr_path.argtypes = [C.c_int, i64, vp, i64, i64, vp, i64, i64, C.c_int, i64, i64]
-        lib.b200sddmm_bsr_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int]
-        lib.b200spmm_bsr.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, i64, i64, vp, vp, vp, C.c_int32, C.c_int, vp, vp, C.c_int,
-                                     vp, i64, i64, vp, i64, C.c_int, C.c_int, i64, i64, i64, i64, i64, vp, C.c_size_t]
-        lib.b200spmm_bsr_workspace_bytes.argtypes = [C.c_int, i64, i64, i64, i64, C.c_int]
-        lib.b200spmm_bsr_workspace_bytes.restype = C.c_size_t
-        lib.b200spmm_bsr_path.argtypes = [C.c_int, i64, C.c_int, vp, vp, i64, i64, C.c_int, i64, i64]
-        lib.b200spmm_bsr_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
-        lib.b200spmm_csr16.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, i64, i64, vp,
-                                       i64, C.c_int, vp, C.c_size_t]
-        lib.b200spmm_csr16_workspace_bytes.argtypes = [i64, i64, i64, i64, i64]
-        lib.b200spmm_csr16_workspace_bytes.restype = C.c_size_t
-        lib.b200spmm_csr16_path.argtypes = [i64, vp, i64, i64]
-        lib.b200spmm_csr16_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
-        lib.b200spmm_csr_t.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, i64, i64, vp,
-                                       i64, C.c_int, C.c_int, vp, C.c_size_t]
-        lib.b200spmm_csr_t_plan.argtypes = [vp, i64, i64, i64, vp, vp, C.c_int32, vp, C.c_size_t]
-        lib.b200spmm_csr_t_layout.argtypes = [C.c_int, i64, i64, i64, i64, i64, i64, vp]
-        lib.b200spmm_csr_t_layout.restype = C.c_size_t
-        lib.b200spmm_csr_t_workspace_bytes.argtypes = [C.c_int, i64, i64, i64, i64, i64, i64]
-        lib.b200spmm_csr_t_workspace_bytes.restype = C.c_size_t
-        lib.b200spmm_csr_t_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]
-        lib.b200spmv_plan_trusted.argtypes = [vp, vp, C.c_int]
-        lib.b200csr2csc.argtypes = [vp, i64, i64, i64, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int32, vp, C.c_size_t]
-        lib.b200csr2csc_workspace_bytes.argtypes = [i64, i64, i64]
-        lib.b200csr2csc_workspace_bytes.restype = C.c_size_t
-        lib.b200coosort.argtypes = [vp, C.c_int, i64, i64, i64, vp, vp, vp, vp, C.c_size_t]
-        lib.b200coosort_workspace_bytes.argtypes = [i64, i64, i64]
-        lib.b200coosort_workspace_bytes.restype = C.c_size_t
-        lib.b200coo2csr.argtypes = [vp, vp, i64, i64, vp, C.c_int32]
-        lib.b200csr2coo.argtypes = [vp, vp, i64, i64, vp, C.c_int32]
-        lib.b200identity_permutation.argtypes = [vp, i64, vp]
-        lib.b200conv_route.argtypes = [C.c_int, i64, i64, i64, C.c_int, C.c_int, vp]
-        lib.b200csr2dense.argtypes = [vp, C.c_int, i64, i64, i64, vp, vp, vp, C.c_int, C.c_int32, vp, i64, C.c_int]
-        lib.b200coo2dense.argtypes = [vp, i64, i64, i64, vp, vp, vp, C.c_int, C.c_int32, vp, i64, C.c_int]
-        lib.b200bell2dense.argtypes = [vp, i64, i64, i64, i64, vp, vp, C.c_int, C.c_int32, vp, i64, C.c_int]
-        lib.b200dense2csr.argtypes = [vp, C.c_int, i64, i64, i64, vp, i64, C.c_int, C.c_int, vp, vp, vp, C.c_int32]
-        lib.b200dense2bell.argtypes = [vp, i64, i64, i64, i64, vp, i64, C.c_int, C.c_int, vp, vp, C.c_int32]
-        lib.b200dense_route.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, i64, i64, i64, C.c_int, C.c_int, i64]
-        lib.b200spmv_csr16.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, vp, vp, C.c_size_t]
-        lib.b200spmv_csr16_workspace_bytes.argtypes = [i64, i64]
-        lib.b200spmv_csr16_workspace_bytes.restype = C.c_size_t
-        lib.b200spmv_csr16_path.argtypes = [vp, vp]
-        lib.b200spmv_csr16_route.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int]
-        lib.b200spmv_route.argtypes = [C.c_int] * 9 + [i64] * 3
-        lib.b200spmv_csr_z.argtypes = [vp, C.c_int, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, vp, vp, C.c_size_t]
-        lib.b200spmv_csr_z_workspace_bytes.argtypes = [i64, i64]
-        lib.b200spmv_csr_z_workspace_bytes.restype = C.c_size_t
-        lib.b200spmv_csr_z_params.argtypes = [vp, vp, vp]
-        lib.b200spsm_csr_workspace_bytes.argtypes = [i64, i64, C.c_int]
-        lib.b200spsm_csr_workspace_bytes.restype = C.c_size_t
-        lib.b200spsm_csr_layout.argtypes = [i64, i64, C.c_int, vp]
-        lib.b200spsm_csr_analysis.argtypes = [vp, i64, i64, vp, vp, C.c_int32, C.c_int, C.c_int, C.c_int, vp, vp, vp]
-        lib.b200spsm_csr_solve.argtypes = [vp, C.c_int, i64, i64, C.c_int, vp, vp, vp, C.c_int, i64, vp, i64, i64, vp, i64, i64, vp]
-        lib.b200spsm_csr_tile.argtypes = [i64, C.c_int]
-        lib.b200spsm_route.argtypes = [C.c_int] * 12 + [i64] * 4 + [C.c_int, C.c_int]
-        _shim = lib
+        _shim = load(path)
     return _shim
 
 
@@ -164,11 +134,7 @@ def spsv() -> C.CDLL:
         if not os.path.exists(path):
             raise RuntimeError(f"{path} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_90a). "
                                "There is no CPU fallback.")
-        lib = C.CDLL(path, mode=C.RTLD_LOCAL)
-        lib.b200spsv_csr_workspace_bytes.restype = C.c_size_t
-        lib.b200spsv_csr_workspace_bytes.argtypes = [C.c_int64, C.c_int64, C.c_int]
-        lib.b200spsv_version.restype = C.c_char_p
-        _spsv = lib
+        _spsv = load(path, header="b200spsv.h")
     return _spsv
 
 
@@ -179,5 +145,5 @@ def gen() -> C.CDLL:
         path = _build.GEN_LIB_PATH
         if not os.path.exists(path):
             raise RuntimeError(f"{path} is missing: run `python -c 'import __graft_entry__ as g; g.build()'`")
-        _gen = C.CDLL(path, mode=C.RTLD_LOCAL)
+        _gen = load(path, header="b200gen.h")
     return _gen

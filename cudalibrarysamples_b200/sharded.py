@@ -27,6 +27,7 @@ same code with the CPU oracle, while bench.py passes the sm_90a operator.
 """
 from __future__ import annotations
 
+import ctypes as C
 import os
 from typing import Callable
 
@@ -209,9 +210,8 @@ class ShardedCsr:
             for t in self.sym:
                 t.zero_()
             # flags of the device-side barrier (csrc/peer_sync.cu): one 8-byte slot per rank in every rank's buffer
-            import ctypes as C
             from . import lib as _lib
-            self._C, self._L = C, _lib.shim()
+            self._L = _lib.shim()
             self.flags = symm.empty(self.world, dtype=torch.int64, device=self.val.device)
             self.flags.zero_()
             torch.cuda.synchronize()
@@ -292,9 +292,8 @@ class ShardedCsr:
                 self.sym[i].copy_(x_shard)                       # (a caller that produces its shard in shard_buffer() skips this)
             # every rank's shard i is written (and step k-1 is fully read): device-side barrier over NVLink peer memory,
             # epoch in device memory -> correct on every replay of a captured step; a missing rank traps after 30 s
-            rc = self._L.b200peer_barrier(self._C.c_void_p(main.cuda_stream), self._C.c_void_p(self.flag_ptrs.data_ptr()),
-                                          self._C.c_void_p(self.epoch.data_ptr()), self._C.c_int(self.rank), self._C.c_int(self.world),
-                                          self._C.c_double(30.0))
+            rc = self._L.b200peer_barrier(main.cuda_stream, self.flag_ptrs.data_ptr(), self.epoch.data_ptr(), self.rank, self.world,
+                                          30.0)
             if rc != 0:
                 raise RuntimeError(f"b200peer_barrier failed with code {rc}")
             self.ev_ready.record(main)
@@ -309,9 +308,8 @@ class ShardedCsr:
                 with torch.cuda.stream(st):
                     if self.sm_pull_ctas > 0:
                         esz = self.x_full.element_size()
-                        rc = self._L.b200peer_pull(self._C.c_void_p(st.cuda_stream), self._C.c_void_p(self.x_full.data_ptr() + h * blk * esz),
-                                                   self._C.c_void_p(self.peer[i][h].data_ptr()), self._C.c_size_t(blk * esz),
-                                                   self._C.c_int(self.sm_pull_ctas))
+                        rc = self._L.b200peer_pull(st.cuda_stream, self.x_full.data_ptr() + h * blk * esz, self.peer[i][h].data_ptr(),
+                                                   blk * esz, self.sm_pull_ctas)
                         if rc != 0:
                             raise RuntimeError(f"b200peer_pull failed with code {rc}")
                     else:
@@ -410,15 +408,13 @@ class ShardedCsr:
             ok = (not self.panels) and self.val.is_cuda and self.rows > 0 and (self.rows == self.x_block or self.world == 1)
             if ok:
                 try:
-                    import ctypes as C
                     from . import lib as _lib
                     L = _lib.shim()
-                    L.b200spmv_csr_short_dot_workspace_bytes.restype = C.c_size_t
                     longest = int((self.off[1:] - self.off[:-1]).max().item())
-                    ok = longest <= int(L.b200spmv_csr_short_max_row())
+                    ok = longest <= L.b200spmv_csr_short_max_row()
                     if ok:
-                        self._dotL, self._dotC = L, C
-                        self._dot_ws = torch.zeros(int(L.b200spmv_csr_short_dot_workspace_bytes()), dtype=torch.uint8, device=self.val.device)
+                        self._dotL = L
+                        self._dot_ws = torch.zeros(L.b200spmv_csr_short_dot_workspace_bytes(), dtype=torch.uint8, device=self.val.device)
                 except Exception:
                     ok = False
             self._fuse_dot = bool(ok)
@@ -428,16 +424,13 @@ class ShardedCsr:
         """y_shard = A[r0:r1, :] @ x  and  dot_out[0] = y_shard . x_shard (this rank's part; fp64, device memory) in one pass
         over the local matrix: T = A*P together with T . P of a CG iteration (cg_example.c:220-227)."""
         assert self.can_fuse_dot()
-        C, L = self._dotC, self._dotL
         self.gather_x(x_shard)
         one = (C.c_double if self.val.dtype == torch.float64 else C.c_float)(1.0)
         zero = (C.c_double if self.val.dtype == torch.float64 else C.c_float)(0.0)
-        rc = L.b200spmv_csr_short_mv_dot(C.c_void_p(torch.cuda.current_stream().cuda_stream), C.c_int(1 if self.val.dtype == torch.float64 else 0),
-                                         C.c_int64(self.rows), C.c_int64(self.cols_padded), C.c_int64(self.nnz),
-                                         C.c_void_p(self.off.data_ptr()), C.c_void_p(self.col.data_ptr()), C.c_void_p(self.val.data_ptr()),
-                                         C.c_int32(0), C.byref(one), C.byref(zero), C.c_int(0), C.c_void_p(self.x_full.data_ptr()),
-                                         C.c_void_p(y_shard.data_ptr()), C.c_void_p(x_shard.data_ptr()), C.c_void_p(dot_out.data_ptr()),
-                                         C.c_void_p(self._dot_ws.data_ptr()))
+        rc = self._dotL.b200spmv_csr_short_mv_dot(torch.cuda.current_stream().cuda_stream, 1 if self.val.dtype == torch.float64 else 0,
+                                                  self.rows, self.cols_padded, self.nnz, self.off.data_ptr(), self.col.data_ptr(),
+                                                  self.val.data_ptr(), 0, C.byref(one), C.byref(zero), 0, self.x_full.data_ptr(),
+                                                  y_shard.data_ptr(), x_shard.data_ptr(), dot_out.data_ptr(), self._dot_ws.data_ptr())
         if rc != 0:
             raise RuntimeError(f"b200spmv_csr_short_mv_dot failed with code {rc}")
         return y_shard

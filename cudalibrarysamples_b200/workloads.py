@@ -9,7 +9,6 @@ full-size matrices never cross PCIe.  torch is plumbing here (memory, sort, cums
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 
 import torch
@@ -21,7 +20,7 @@ RMAT_OVERSAMPLE = 1.5
 
 
 def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    return torch.cuda.current_stream().cuda_stream
 
 
 def _check(rc, what):
@@ -45,8 +44,7 @@ def rmat_scale(n):
 
 def uniform(seed, count, dtype=torch.float64, device="cuda", i0=0):
     out = torch.empty(count, dtype=dtype, device=device)
-    _check(_lib.gen().b200gen_uniform(_stream(), C.c_int(_dt(dtype)), C.c_uint64(seed), C.c_int64(i0), C.c_int64(count),
-                                       C.c_void_p(out.data_ptr())), "b200gen_uniform")
+    _check(_lib.gen().b200gen_uniform(_stream(), _dt(dtype), seed, i0, count, out.data_ptr()), "b200gen_uniform")
     return out
 
 
@@ -62,9 +60,8 @@ def rmat_csr(rows, cols=None, avg_nnz=16, seed=42, val_seed=43, dtype=torch.floa
     L = _lib.gen()
     for e0 in range(0, cand, chunk):
         n = min(chunk, cand - e0)
-        _check(L.b200gen_rmat_keys(_stream(), C.c_uint64(seed), C.c_int64(e0), C.c_int64(n), C.c_int32(scale), C.c_uint64(tA),
-                                   C.c_uint64(tAB), C.c_uint64(tABC), C.c_int64(rows), C.c_int64(cols),
-                                   C.c_void_p(keys.data_ptr() + 8 * e0)), "b200gen_rmat_keys")
+        _check(L.b200gen_rmat_keys(_stream(), seed, e0, n, scale, tA, tAB, tABC, rows, cols, keys.data_ptr() + 8 * e0),
+               "b200gen_rmat_keys")
     # first occurrence of every valid key, in stream order
     skeys, perm = torch.sort(keys, stable=True)
     del keys
@@ -94,14 +91,13 @@ def stencil5_csr(grid, mass=0.04, ux=0.0, uy=0.0, device="cuda"):
     n = grid * grid
     L = _lib.gen()
     counts = torch.empty(n, dtype=torch.int32, device=device)
-    _check(L.b200gen_stencil5_counts(_stream(), C.c_int32(grid), C.c_void_p(counts.data_ptr())), "stencil5_counts")
+    _check(L.b200gen_stencil5_counts(_stream(), grid, counts.data_ptr()), "stencil5_counts")
     off = torch.zeros(n + 1, dtype=torch.int32, device=device)
     off[1:] = torch.cumsum(counts, 0, dtype=torch.int64).to(torch.int32)
     nnz = 5 * n - 4 * grid
     col = torch.empty(nnz, dtype=torch.int32, device=device)
     val = torch.empty(nnz, dtype=torch.float64, device=device)
-    _check(L.b200gen_stencil5_fill(_stream(), C.c_int32(grid), C.c_double(mass), C.c_double(ux), C.c_double(uy),
-                                   C.c_void_p(off.data_ptr()), C.c_void_p(col.data_ptr()), C.c_void_p(val.data_ptr())),
+    _check(L.b200gen_stencil5_fill(_stream(), grid, mass, ux, uy, off.data_ptr(), col.data_ptr(), val.data_ptr()),
            "stencil5_fill")
     return off, col, val
 
@@ -111,14 +107,14 @@ def laplace7_csr(nx, dtype=torch.float64, device="cuda"):
     n = nx ** 3
     L = _lib.gen()
     counts = torch.empty(n, dtype=torch.int32, device=device)
-    _check(L.b200gen_laplace7_counts(_stream(), C.c_int32(nx), C.c_void_p(counts.data_ptr())), "laplace7_counts")
+    _check(L.b200gen_laplace7_counts(_stream(), nx, counts.data_ptr()), "laplace7_counts")
     off = torch.zeros(n + 1, dtype=torch.int32, device=device)
     off[1:] = torch.cumsum(counts, 0, dtype=torch.int64).to(torch.int32)
     nnz = int(off[-1].item())
     col = torch.empty(nnz, dtype=torch.int32, device=device)
     val = torch.empty(nnz, dtype=dtype, device=device)
-    _check(L.b200gen_laplace7_fill(_stream(), C.c_int(_dt(dtype)), C.c_int32(nx), C.c_void_p(off.data_ptr()),
-                                   C.c_void_p(col.data_ptr()), C.c_void_p(val.data_ptr())), "laplace7_fill")
+    _check(L.b200gen_laplace7_fill(_stream(), _dt(dtype), nx, off.data_ptr(), col.data_ptr(), val.data_ptr()),
+           "laplace7_fill")
     return off, col, val
 
 

@@ -151,19 +151,15 @@ def ours_fn(rows, cols, row, col, val, n, Bs, ldb, Cs, ldc, order, op, batches=1
 def csr_fn(rows, cols, off, col, val, n, Bs, ldb, Cs, ldc, order):
     lib = _lib.shim()
     dt = 1 if val.dtype == torch.float64 else 0
-    lib.b200spmm_csr_workspace_bytes.restype = C.c_size_t
-    wsb = lib.b200spmm_csr_workspace_bytes(C.c_int(dt), C.c_int64(cols), C.c_int64(n), C.c_int(int(order == ROW)))
+    wsb = lib.b200spmm_csr_workspace_bytes(dt, cols, n, int(order == ROW))
     ws = torch.empty(max(wsb, 16), dtype=torch.uint8, device=DEV)
     sc = cs._CT[val.dtype]
     a1, b0 = sc(1.0), sc(0.0)
-    i64 = C.c_int64
 
     def fn(_keep=(ws, a1, b0)):
-        rc = lib.b200spmm_csr_ws(C.c_void_p(torch.cuda.current_stream().cuda_stream), C.c_int(dt), i64(rows), i64(cols), i64(n),
-                                 i64(col.numel()), C.c_void_p(off.data_ptr()), C.c_void_p(col.data_ptr()), C.c_void_p(val.data_ptr()),
-                                 C.c_int32(0), C.c_void_p(C.addressof(a1)), C.c_void_p(C.addressof(b0)), C.c_int(0),
-                                 C.c_void_p(Bs.data_ptr()), i64(ldb), C.c_int(int(order == ROW)), C.c_void_p(Cs.data_ptr()), i64(ldc),
-                                 C.c_int(int(order == ROW)), C.c_void_p(ws.data_ptr()))
+        rc = lib.b200spmm_csr_ws(torch.cuda.current_stream().cuda_stream, dt, rows, cols, n, col.numel(), off.data_ptr(), col.data_ptr(),
+                                 val.data_ptr(), 0, C.addressof(a1), C.addressof(b0), 0, Bs.data_ptr(), ldb, int(order == ROW),
+                                 Cs.data_ptr(), ldc, int(order == ROW), ws.data_ptr())
         assert rc == 0, rc
     return fn
 

@@ -170,10 +170,7 @@ def run_case(name, rows, cols, off, col, val32, dt, yt, seed=1, variants=()):
     row["share_of_datasheet_3.35TBs"] = b / t / PEAK_BYTES
     row["bound_us"] = b / PEAK_BYTES * 1e6
     for path in variants:                   # the same call on another build of the library (same ABI)
-        V = C.CDLL(path, mode=C.RTLD_LOCAL)
-        V.b200spmv_csr16.argtypes = L.b200spmv_csr16.argtypes
-        V.b200spmv_csr16_workspace_bytes.argtypes = [C.c_int64, C.c_int64]
-        V.b200spmv_csr16_workspace_bytes.restype = C.c_size_t
+        V = _lib.load(path)
         wsb = V.b200spmv_csr16_workspace_bytes(rows, nnz)
         ws = torch.empty(max(wsb, 16), dtype=torch.uint8, device=DEV)
         vy = torch.zeros_like(ours_y)

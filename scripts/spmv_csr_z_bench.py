@@ -193,10 +193,7 @@ def run_case(name, rows, cols, off, col, vals, op, beta, seed=1, variants=()):
     row["share_of_datasheet_3.35TBs"] = b / t / PEAK_BYTES
     row["bound_us"] = b / PEAK_BYTES * 1e6
     for path in (variants if op == NT else ()):     # the same call on another build of the library (same ABI)
-        V = C.CDLL(path, mode=C.RTLD_LOCAL)
-        V.b200spmv_csr_z.argtypes = L.b200spmv_csr_z.argtypes
-        V.b200spmv_csr_z_workspace_bytes.argtypes = [C.c_int64, C.c_int64]
-        V.b200spmv_csr_z_workspace_bytes.restype = C.c_size_t
+        V = _lib.load(path)
         vwsb = V.b200spmv_csr_z_workspace_bytes(rows, nnz)
         vws = torch.empty(max(vwsb, 16), dtype=torch.uint8, device=DEV)
         vy = y0.clone()

@@ -34,21 +34,19 @@ for wl in sys.argv[2:] or ["rmat1m"]:
         path = os.path.join(VDIR, f"libb200spmv_{tag}.so")
         api = cs.Api("b200", lib_path=path)
         op = cs.SpMVOperator(api, "csr", rows, rows, dict(off=off, col=col, val=val))
-        nt = api.lib.b200spmv_csr_num_tiles
-        nt.restype = C.c_int64
-        ntiles = nt(C.c_int64(rows), C.c_int64(int(col.numel())))
+        ntiles = api.lib.b200spmv_csr_num_tiles(rows, col.numel())
         y = torch.zeros(rows, dtype=torch.float64, device="cuda")
         for _ in range(3):
             op(x, y)
         trace = torch.zeros(ntiles * 4, dtype=torch.int64, device="cuda")
+        # only -DB200_CSR_TRACE builds define this hook, so no header declares it: the pointer goes as an explicit c_void_p
         api.lib.b200spmv_debug_set_trace(C.c_void_p(trace.data_ptr()))
         op(x, y)
         torch.cuda.synchronize()
         api.lib.b200spmv_debug_set_trace(C.c_void_p(0))
         t = trace.cpu().numpy().reshape(-1, 4)
-        o = api.lib.b200spmv_csr_plan_tiles_offset
-        o.restype = C.c_size_t
-        tiles = op.buffer[o():o() + (ntiles + 1) * 8].view(torch.int32).view(-1, 2).cpu().numpy().astype(np.int64)
+        o = api.lib.b200spmv_csr_plan_tiles_offset()
+        tiles = op.buffer[o:o + (ntiles + 1) * 8].view(torch.int32).view(-1, 2).cpu().numpy().astype(np.int64)
         trows = np.diff(tiles[:, 0]); tnnz = np.diff(tiles[:, 1])
         d1 = t[:, 1] - t[:, 0]; d2 = t[:, 2] - t[:, 1]; dt = t[:, 2] - t[:, 0]
         print(f"== {wl} {tag}: tiles={ntiles}")

@@ -4,15 +4,16 @@ import os
 import re
 import subprocess
 
+import pytest
+
+from cudalibrarysamples_b200 import build
+from cudalibrarysamples_b200.lib import load, prototypes, signatures
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, "include", "b200spmv.h")
-GEN_HEADER = os.path.join(ROOT, "include", "b200gen.h")
 
 
-def declared_symbols(header=HEADER, tag="B200SPMV_EXPORT"):
-    text = open(header).read()
-    names = re.findall(tag + r"\s+[\w\s\*]+?\b(\w+)\s*\(", text)
-    return sorted(set(names))
+def declared_symbols(header="b200spmv.h"):
+    return sorted({name for _, name, _ in prototypes(header)})
 
 
 def exported(lib):
@@ -38,17 +39,16 @@ def test_library_exports_every_declared_symbol(built_lib):
 
 def test_bench_plumbing_is_not_part_of_the_product_abi(built_lib):
     """The synthetic-workload generators live in libb200gen.so (include/b200gen.h); libb200spmv.so exports none of them."""
-    from cudalibrarysamples_b200 import build
     assert not [n for n in exported(built_lib) if n.startswith("b200gen")]
     assert not [n for n in declared_symbols() if n.startswith("b200gen")]
-    gen = declared_symbols(GEN_HEADER, "B200GEN_EXPORT")
+    gen = declared_symbols("b200gen.h")
     assert len(gen) >= 6
     have = exported(build.GEN_LIB_PATH)
     assert not [n for n in gen if n not in have]
 
 
 def test_options_are_set_through_the_abi_not_the_environment(built_lib):
-    lib = ctypes.CDLL(built_lib)
+    lib = load(built_lib)
     assert lib.b200spmv_set_option(b"B200SPMV_CSR_KERNEL", b"seg") == 0
     assert lib.b200spmv_set_option(b"B200SPMV_CSR_KERNEL", b"auto") == 0
     assert lib.b200spmv_set_option(b"B200SPMV_CSR_KERNEL", b"no-such-kernel") == -1
@@ -67,11 +67,8 @@ def test_options_are_set_through_the_abi_not_the_environment(built_lib):
 
 
 def test_library_loads_without_a_gpu(built_lib):
-    lib = ctypes.CDLL(built_lib)
-    lib.b200spmv_version.restype = ctypes.c_char_p
+    lib = load(built_lib)
     assert b"sm_90a" in lib.b200spmv_version()
-    lib.b200spmv_csr_workspace_bytes.restype = ctypes.c_size_t
-    lib.b200spmv_csr_num_tiles.restype = ctypes.c_int64
     t, l, b = ctypes.c_int32(), ctypes.c_int32(), ctypes.c_int32()
     lib.b200spmv_csr_plan_params(ctypes.byref(t), ctypes.byref(l), ctypes.byref(b))
     assert t.value > l.value > 0 and b.value % 32 == 0
@@ -83,11 +80,62 @@ def test_library_loads_without_a_gpu(built_lib):
     blk, max_ctas = ctypes.c_int32(), ctypes.c_int32()
     lib.b200cg_params(ctypes.byref(blk), ctypes.byref(max_ctas))
     assert blk.value % 32 == 0 and max_ctas.value > 0
-    lib.b200cg_workspace_bytes.restype = ctypes.c_size_t
     assert lib.b200cg_workspace_bytes() == (max_ctas.value + 2) * 8
     # argument validation happens on the host, before any CUDA call
     assert lib.b200spmv_csr_mv(None, 7, ctypes.c_int64(4), ctypes.c_int64(4), ctypes.c_int64(9), None, None, None, 0,
                                None, None, 0, None, None, None) == -1
+
+
+HEADERS = [("b200spmv.h", build.LIB_PATH), ("b200spsv.h", build.SPSV_LIB_PATH), ("b200gen.h", build.GEN_LIB_PATH)]
+
+
+@pytest.mark.parametrize("header", [h for h, _ in HEADERS])
+def test_every_b200_prototype_has_a_ctypes_signature(header):
+    """each B200*_EXPORT tag of the header starts a prototype the parser reads, and every b200* one maps to ctypes types"""
+    with open(os.path.join(ROOT, "include", header)) as f:
+        text = re.sub(r"/\*.*?\*/", " ", f.read(), flags=re.S)
+    tags = len(re.findall(r"\bB200\w*_EXPORT\b", text)) - 1                # minus its #define
+    assert len(prototypes(header)) == tags
+    assert sorted(signatures(header)) == [n for n in declared_symbols(header) if n.startswith("b200")]
+
+
+@pytest.mark.parametrize("header, path", HEADERS)
+def test_declared_and_exported_b200_functions_are_the_same(built_lib, header, path):
+    load(path, header=header)                                                # resolves every declared name, or raises
+    assert {n for n in exported(path) if n.startswith("b200")} == set(signatures(header))
+
+
+def test_signatures_follow_the_header():
+    spmv, gen = signatures("b200spmv.h"), signatures("b200gen.h")
+    i32, i64 = ctypes.c_int, ctypes.c_int64
+    assert spmv["b200spmv_csr_workspace_bytes"] == (ctypes.c_size_t, [i64, i64])
+    assert spmv["b200spmv_version"] == (ctypes.c_char_p, [])
+    assert gen["b200gen_stencil5_fill"][1][2:5] == [ctypes.c_double] * 3
+    assert spmv["b200spmm_coo_workspace_bytes"] == (ctypes.c_size_t, [i32, i32, i64, i64, i64, i64, i32, i32, i64])
+
+
+def test_declarations_are_live(built_lib):
+    lib = load(built_lib)
+    with pytest.raises(ctypes.ArgumentError):                                # an int64_t where the header says int
+        lib.b200spmm_coo_workspace_bytes(ctypes.c_int64(0), 0, 100, 80, 8, 1000, 1, 1, 0)
+    nnz = 1 << 40                                                            # plain ints, a size_t result past 2^32
+    nt = lib.b200spmv_csr_num_tiles(1000, nnz)
+    ws = lib.b200spmv_csr_workspace_bytes(1000, nnz)
+    assert ws > 1 << 32 and ws >= (nt + 1) * (8 + 4 + 8 + 8)
+
+
+def test_only_lib_py_declares_native_signatures():
+    """every b200* signature comes from lib.load(); the checker's own oracle library declares its few functions itself"""
+    allowed = {os.path.join("cudalibrarysamples_b200", "lib.py"), os.path.join("oracle", "oracle.py")}
+    found = []
+    for d, dirs, files in os.walk(ROOT):
+        dirs[:] = [x for x in dirs if not x.startswith(".") and x != "__pycache__"]
+        for name in files:
+            rel = os.path.relpath(os.path.join(d, name), ROOT)
+            if name.endswith(".py") and rel not in allowed:
+                with open(os.path.join(d, name)) as f:
+                    found += [f"{rel}:{i}" for i, line in enumerate(f, 1) if re.search(r"\b(argtypes|restype)\s*=(?!=)", line)]
+    assert not found, found
 
 
 def kernel_sass(built_lib, pattern):

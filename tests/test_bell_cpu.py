@@ -11,6 +11,7 @@ import textwrap
 import numpy as np
 import pytest
 
+from cudalibrarysamples_b200.lib import load
 from oracle import bell_ref as R
 from test_abi import declared_symbols, exported
 
@@ -79,10 +80,11 @@ def test_exactness_precondition():
 
 
 ROUTE = textwrap.dedent("""
-    import ctypes as C, sys
+    import ctypes as C, os, sys
+    sys.path.insert(0, os.path.dirname(os.path.dirname(sys.argv[1])))     # the repository: argv[1] is its built library
+    from cudalibrarysamples_b200.lib import load
     real = C.CDLL(sys.argv[2], mode=C.RTLD_GLOBAL)
-    shim = C.CDLL(sys.argv[1])
-    shim.b200spmm_bell_route.argtypes = [C.c_void_p] * 3 + [C.c_int] * 4
+    shim = load(sys.argv[1])
     I32, I64 = 2, 3
     F32, F64, F16, BF16, I8 = 0, 1, 2, 14, 3
     ROW, COL = 2, 1
@@ -152,10 +154,7 @@ def test_route_table_over_real_descriptors(built_lib, mode):
 
 
 def test_host_side_argument_rejection(built_lib):
-    lib = C.CDLL(built_lib)
-    lib.b200spmm_bell.argtypes = [C.c_void_p, C.c_int, C.c_int] + [C.c_int64] * 5 + [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
-                                                                                       C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int,
-                                                                                       C.c_void_p, C.c_int64, C.c_int]
+    lib = load(built_lib)
     one = C.c_float(1.0)
     dummy = (C.c_int * 64)()
     p = C.addressof(dummy)
@@ -176,7 +175,7 @@ def test_host_side_argument_rejection(built_lib):
 
 
 def test_params(built_lib):
-    P = R.params(C.CDLL(built_lib))
+    P = R.params(load(built_lib))
     assert P["n_tile"] % 16 == 0 and P["stages"] >= 2 and P["max_rows_per_cta"] % 16 == 0
 
 

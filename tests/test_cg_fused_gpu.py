@@ -31,7 +31,6 @@ SLOT = {"delta": 0, "denom": 1, "delta_new": 2, "out": 3}
 def L():
     from cudalibrarysamples_b200 import lib as _lib
     lib = _lib.shim()
-    lib.b200cg_workspace_bytes.restype = C.c_size_t
     return lib
 
 

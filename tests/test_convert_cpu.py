@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 import scipy.sparse as sp
 
+from cudalibrarysamples_b200.lib import load
 from oracle import convert_ref as R
 from oracle import oracle as O
 from test_abi import declared_symbols, exported
@@ -19,7 +20,6 @@ NEW = ["b200csr2csc", "b200csr2csc_workspace_bytes", "b200coosort", "b200coosort
        "b200identity_permutation", "b200conv_route", "cusparseCsr2cscEx2_bufferSize", "cusparseCsr2cscEx2",
        "cusparseXcoosort_bufferSizeExt", "cusparseXcoosortByRow", "cusparseXcoosortByColumn", "cusparseXcoo2csr", "cusparseXcsr2coo",
        "cusparseCreateIdentityPermutation"]
-i64, vp = C.c_int64, C.c_void_p
 
 
 def test_header_declares_and_library_exports_the_conversion_symbols(built_lib):
@@ -96,22 +96,8 @@ def test_coo2csr_and_csr2coo_restatement(base):
         assert np.array_equal(R.coo2csr(coo, rows, base), np.asarray(off) + base), name
 
 
-def _lib(built_lib):
-    lib = C.CDLL(built_lib)
-    lib.b200csr2csc.argtypes = [vp, i64, i64, i64, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int32, vp, C.c_size_t]
-    lib.b200csr2csc_workspace_bytes.argtypes = [i64, i64, i64]
-    lib.b200csr2csc_workspace_bytes.restype = C.c_size_t
-    lib.b200coosort.argtypes = [vp, C.c_int, i64, i64, i64, vp, vp, vp, vp, C.c_size_t]
-    lib.b200coosort_workspace_bytes.argtypes = [i64, i64, i64]
-    lib.b200coosort_workspace_bytes.restype = C.c_size_t
-    lib.b200coo2csr.argtypes = [vp, vp, i64, i64, vp, C.c_int32]
-    lib.b200csr2coo.argtypes = [vp, vp, i64, i64, vp, C.c_int32]
-    lib.b200identity_permutation.argtypes = [vp, i64, vp]
-    return lib
-
-
 def test_workspace_formulas(built_lib):
-    lib = _lib(built_lib)
+    lib = load(built_lib)
     for m, n, nnz in ((1000, 700, 5000), (5, 1, 4), (10, 10, 0), (1 << 20, 1 << 20, 16 << 20), (10 << 20, 10 << 20, 160 << 20), (0, 0, 0)):
         assert lib.b200csr2csc_workspace_bytes(m, n, nnz) == R.workspace("csr2csc", nnz)
         assert lib.b200coosort_workspace_bytes(m, n, nnz) == R.workspace("coosort", nnz)
@@ -121,7 +107,7 @@ def test_workspace_formulas(built_lib):
 
 
 def test_host_side_argument_rejection(built_lib):
-    lib = _lib(built_lib)
+    lib = load(built_lib)
     big = (C.c_byte * (1 << 20))()
     p = (C.addressof(big) + 255) // 256 * 256
     wsb = (1 << 20) - 256
@@ -154,9 +140,10 @@ def test_host_side_argument_rejection(built_lib):
 
 
 ROUTE = textwrap.dedent(r"""
-    import ctypes as C, sys
-    shim = C.CDLL(sys.argv[1])
-    shim.b200conv_route.argtypes = [C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_void_p]
+    import ctypes as C, os, sys
+    sys.path.insert(0, os.path.dirname(os.path.dirname(sys.argv[1])))     # the repository: argv[1] is its built library
+    from cudalibrarysamples_b200.lib import load
+    shim = load(sys.argv[1])
     forward = sys.argv[2] == "forward"
     native = eval(sys.argv[3])
     buf = (C.c_double * 64)()

@@ -11,9 +11,11 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REAL = "/usr/local/cuda/lib64/libcusparse.so.12"
 
 SCRIPT = textwrap.dedent("""
-    import ctypes as C, sys
+    import ctypes as C, os, sys
+    sys.path.insert(0, os.path.dirname(os.path.dirname(sys.argv[1])))     # the repository: argv[1] is its built library
+    from cudalibrarysamples_b200.lib import load
     real = C.CDLL(sys.argv[2], mode=C.RTLD_GLOBAL)
-    shim = C.CDLL(sys.argv[1])
+    shim = load(sys.argv[1])
     I32, F32, COL = 2, 0, 1
     off = (C.c_int * 5)(0, 3, 4, 7, 9)
     col = (C.c_int * 18)()
@@ -102,8 +104,6 @@ SCRIPT = textwrap.dedent("""
     # the route exports give both the same (native) answer -- a BSR descriptor the shim did not record would be forwarded
     I64, VP, INT = C.c_int64, C.c_void_p, C.c_int
     F16, ROW, NT, TR = 2, 2, 0, 1
-    shim.b200sddmm_route.argtypes = shim.b200sddmm_bsr_route.argtypes = [C.c_void_p] * 3 + [C.c_int] * 3
-    shim.b200spmm_coo_route.argtypes = [C.c_void_p] * 3 + [C.c_int] * 4
     big = (C.c_double * (1 << 20))()
     at = C.addressof
 

@@ -361,7 +361,6 @@ def test_spmm_exact(cs, b200, closed, profiles, kind, order_b, order_c):
 def test_short_mv_dot_exact(b200, profiles, kind):
     """b200spmv_csr_short_mv_dot: y = A x and the fp64 dot y . x, both exact"""
     L = b200.lib
-    L.b200spmv_csr_short_dot_workspace_bytes.restype = C.c_size_t
     f = fixture(profiles, "short_block_caps", kind)
     x = np.resize(f.x, max(f.rows, f.cols))[:f.cols]
     w = E.values(kind, 0, f.rows, 0, 5)[1]

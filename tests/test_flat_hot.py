@@ -81,7 +81,6 @@ def test_hot_plan_reference_invariants():
 def _lib():
     from cudalibrarysamples_b200 import lib
     L = lib.shim()
-    L.b200spmv_csr_flat_workspace_bytes.restype = C.c_size_t
     return L
 
 

@@ -568,7 +568,6 @@ def test_fused_cg_graph_replay_gives_the_eager_bits(cs, b200, fuse_dot):
         return cs.SpMVOperator(b200, "csr", rr, cc, arrays, preprocess=True)
     sh = ShardedCsr(dev(off), dev(col), dev(val), 0, 1, make_local, balance="rows")
     L = _lib.shim()
-    L.b200cg_workspace_bytes.restype = C.c_size_t
     ws = torch.zeros(int(L.b200cg_workspace_bytes()), dtype=torch.uint8, device="cuda")
     bb = torch.full((1,), float("nan"), dtype=torch.float64, device="cuda")
     assert L.b200cg_dot(C.c_void_p(torch.cuda.current_stream().cuda_stream), C.c_int64(n), C.c_void_p(b.data_ptr()),
@@ -734,7 +733,6 @@ def test_flat_plan_is_bit_exact(case, base):
     from cudalibrarysamples_b200 import lib
     from oracle.partition_ref import flat_plan
     L = lib.shim()
-    L.b200spmv_csr_flat_workspace_bytes.restype = C.c_size_t
     if case == "rmat":
         off = O.rmat_csr(200000, avg_nnz=16, seed=5, val_seed=6)[0]
     elif case == "stencil":
@@ -894,7 +892,6 @@ def test_short_kernel_with_the_dot_product_in_its_epilogue(b200, dtype):
     accumulated in fp64, deterministic, and the arrival counter of its workspace is left at zero (second call = same bits)."""
     import ctypes as C
     L = b200.lib
-    L.b200spmv_csr_short_dot_workspace_bytes.restype = C.c_size_t
     off, col, val = O.gen_stencil5(257)
     n = 257 * 257
     val = val.astype(NP[dtype])

@@ -6,6 +6,8 @@ import itertools
 
 import pytest
 
+from cudalibrarysamples_b200.lib import load
+
 CSR, CSC, COO, BELL, BSR, SELL = 1, 2, 3, 5, 6, 7
 N, T, H = 0, 1, 2
 I32, I64, U16 = 2, 3, 1
@@ -16,7 +18,7 @@ FORWARD, FAST, GENERIC = 0, 1, 2
 
 @pytest.fixture()
 def lib(built_lib):
-    L = C.CDLL(built_lib)
+    L = load(built_lib)
     yield L
     assert L.b200spmv_set_option(b"B200SPMV_GENERIC", b"csr") == 0      # back to the default
 

@@ -11,6 +11,7 @@ import textwrap
 import numpy as np
 import pytest
 
+from cudalibrarysamples_b200.lib import load
 from oracle import exact as X
 from oracle import sddmm_ref as R
 from test_abi import declared_symbols, exported, kernel_sass
@@ -63,7 +64,7 @@ def test_wide_values_need_more_than_fp32():
 
 
 def test_chunk_walk_computes_every_entry_once(built_lib):
-    lib = C.CDLL(built_lib)
+    lib = load(built_lib)
     P = R.params(lib)
     w = P["warp_chunk"]
     lens = []
@@ -88,7 +89,7 @@ def test_chunk_walk_computes_every_entry_once(built_lib):
 
 
 def test_k_edges_cover_every_group_width(built_lib):
-    P = R.params(C.CDLL(built_lib))
+    P = R.params(load(built_lib))
     for itemsize in (4, 8):
         v = P["vec_bytes"] // itemsize
         ks = R.k_edges(P, itemsize)
@@ -99,9 +100,11 @@ def test_k_edges_cover_every_group_width(built_lib):
 
 
 ROUTE = textwrap.dedent("""
-    import ctypes as C, sys
+    import ctypes as C, os, sys
+    sys.path.insert(0, os.path.dirname(os.path.dirname(sys.argv[1])))     # the repository: argv[1] is its built library
+    from cudalibrarysamples_b200.lib import load
     real = C.CDLL(sys.argv[2], mode=C.RTLD_GLOBAL)
-    shim = C.CDLL(sys.argv[1])
+    shim = load(sys.argv[1])
     I32, I64, F32, F64, F16, C32 = 2, 3, 0, 1, 2, 4
     ROW, COL = 2, 1
     NT, TR, CT = 0, 1, 2
@@ -188,7 +191,7 @@ def test_route_table_over_real_descriptors(built_lib, mode):
 
 
 def test_host_side_argument_rejection(built_lib):
-    lib = C.CDLL(built_lib)
+    lib = load(built_lib)
     one = C.c_float(1.0)
     dummy = (C.c_int * 8)()
 
@@ -210,7 +213,6 @@ def test_host_side_argument_rejection(built_lib):
     assert call(m=1 << 31) == -1 and call(nnz=1 << 31) == -1
     assert call(nnz=0) == 0 and call(m=0, nnz=0) == 0              # nothing to do: no launch
     ws = lib.b200sddmm_csr_workspace_bytes
-    ws.restype = C.c_size_t
     i64 = C.c_int64
     assert ws(0, i64(10), i64(20), i64(8), i64(8), i64(1), i64(1), i64(8), 1, i64(0), i64(0)) == 0          # both K-contiguous
     assert ws(0, i64(10), i64(20), i64(8), i64(8), i64(1), i64(20), i64(1), 1, i64(0), i64(0)) == 768        # B copied: 640 B -> 768

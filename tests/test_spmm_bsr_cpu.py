@@ -11,6 +11,7 @@ import textwrap
 import numpy as np
 import pytest
 
+from cudalibrarysamples_b200.lib import load
 from oracle import spmm_bsr_ref as R
 from test_abi import declared_symbols, exported
 
@@ -67,7 +68,7 @@ PATTERNS = {
 def test_walk_writes_each_entry_once(built_lib, name):
     """both walks: every block-row written exactly once, every stored block multiplied exactly once in its row's piece order, carry
     slots written once and read in ascending piece order by the one fix-up that writes their row"""
-    P = R.params(C.CDLL(built_lib))
+    P = R.params(load(built_lib))
     off, col = PATTERNS[name]()
     bnnz = len(col)
     brows = len(off) - 1
@@ -103,11 +104,11 @@ def test_walk_splits_a_global_row():
 
 
 ROUTE = textwrap.dedent("""
-    import ctypes as C, sys
+    import ctypes as C, os, sys
+    sys.path.insert(0, os.path.dirname(os.path.dirname(sys.argv[1])))     # the repository: argv[1] is its built library
+    from cudalibrarysamples_b200.lib import load
     real = C.CDLL(sys.argv[2], mode=C.RTLD_GLOBAL)
-    shim = C.CDLL(sys.argv[1])
-    shim.b200spmm_bsr_route.argtypes = [C.c_void_p] * 3 + [C.c_int] * 4
-    shim.b200spmm_batch_count.argtypes = [C.c_void_p] * 3
+    shim = load(sys.argv[1])
     I32, I64 = 2, 3
     F32, F64, F16, BF16, C32 = 0, 1, 2, 14, 4
     ROW, COL = 2, 1
@@ -199,10 +200,7 @@ def test_route_table_over_real_descriptors(built_lib, mode):
 
 
 def test_host_side_argument_rejection(built_lib):
-    lib = C.CDLL(built_lib)
-    i64, vp = C.c_int64, C.c_void_p
-    lib.b200spmm_bsr.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, i64, i64, vp, vp, vp, C.c_int32, C.c_int, vp, vp, C.c_int,
-                                 vp, i64, i64, vp, i64, C.c_int, C.c_int, i64, i64, i64, i64, i64, vp, C.c_size_t]
+    lib = load(built_lib)
     one = C.c_float(1.0)
     dummy = (C.c_int * 64)()
     p = C.addressof(dummy)
@@ -227,9 +225,7 @@ def test_host_side_argument_rejection(built_lib):
 
 def test_workspace_bytes(built_lib):
     """two carry slots of bs x n accumulators per chunk of ch stored blocks, per batch matrix"""
-    lib = C.CDLL(built_lib)
-    lib.b200spmm_bsr_workspace_bytes.argtypes = [C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int]
-    lib.b200spmm_bsr_workspace_bytes.restype = C.c_size_t
+    lib = load(built_lib)
     P = R.params(lib)
     for t, m, n, bs, bnnz, batch in ((F16, 4096, 64, 64, 640, 1), (F64, 4096, 64, 64, 640, 1), (F16, 4096, 64, 64, 640, 16),
                                      (BF16, 16384, 128, 16, 100000, 1), (F32, 64, 8, 4, 3, 2)):
@@ -241,9 +237,7 @@ def test_workspace_bytes(built_lib):
 
 
 def test_path_selection(built_lib):
-    lib = C.CDLL(built_lib)
-    i64, vp = C.c_int64, C.c_void_p
-    lib.b200spmm_bsr_path.argtypes = [C.c_int, i64, C.c_int, vp, vp, i64, i64, C.c_int, i64, i64]
+    lib = load(built_lib)
     path = lambda t=F16, bs=32, ar=1, V=4096, B=8192, sbk=64, sbj=1, batch=1, sv=0, sb=0: lib.b200spmm_bsr_path(  # noqa: E731
         t, bs, ar, V, B, sbk, sbj, batch, sv, sb)
     assert path() == 1 and path(t=BF16) == 1
@@ -257,7 +251,7 @@ def test_path_selection(built_lib):
 
 
 def test_params(built_lib):
-    P = R.params(C.CDLL(built_lib))
+    P = R.params(load(built_lib))
     assert P["k_slab"] == 16 and P["k_slab"] * P["slabs_per_stage"] >= 64 and P["stages"] >= 2
     assert P["max_rows_per_cta"] % 16 == 0 and P["chunk_min"] >= 1 and P["chunk_factor"] >= 1 and P["target_ctas"] >= 132
 

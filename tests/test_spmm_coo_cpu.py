@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 import scipy.sparse as sp
 
+from cudalibrarysamples_b200.lib import load
 from oracle import oracle as O
 from oracle import spmm_coo_ref as R
 from test_abi import declared_symbols, exported
@@ -80,7 +81,7 @@ def gpu_structures(chunk):
 def test_chunk_walk_model_at_the_gpu_test_sizes(built_lib):
     """the numpy restatement of the sorted path computes the reference and writes every entry of C once, and the GPU test structures
     reach every edge of the walk"""
-    chunk = R.params(C.CDLL(built_lib))["chunk"]
+    chunk = R.params(load(built_lib))["chunk"]
     seen = {}
     for name, (rows, row) in gpu_structures(chunk).items():
         v, b, c0 = R.values(row.size, 37, rows, 5, seed=len(name))
@@ -101,10 +102,11 @@ def test_chunk_walk_model_at_the_gpu_test_sizes(built_lib):
 
 
 ROUTE = textwrap.dedent("""
-    import ctypes as C, sys
+    import ctypes as C, os, sys
+    sys.path.insert(0, os.path.dirname(os.path.dirname(sys.argv[1])))     # the repository: argv[1] is its built library
+    from cudalibrarysamples_b200.lib import load
     real = C.CDLL(sys.argv[2], mode=C.RTLD_GLOBAL)
-    shim = C.CDLL(sys.argv[1])
-    shim.b200spmm_coo_route.argtypes = [C.c_void_p] * 3 + [C.c_int] * 4
+    shim = load(sys.argv[1])
     I32, I64 = 2, 3
     F32, F64, F16 = 0, 1, 2
     ROW, COL = 2, 1
@@ -187,10 +189,7 @@ def test_route_table_over_real_descriptors(built_lib, mode):
 
 
 def test_host_side_argument_rejection(built_lib):
-    lib = C.CDLL(built_lib)
-    vp, i64 = C.c_void_p, C.c_int64
-    lib.b200spmm_coo.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, i64, C.c_int, vp, i64,
-                                 C.c_int, C.c_int, i64, i64, i64, vp, C.c_size_t]
+    lib = load(built_lib)
     one = C.c_float(1.0)
     dummy = (C.c_int * 64)()
     p = C.addressof(dummy)
@@ -213,11 +212,9 @@ def test_host_side_argument_rejection(built_lib):
 
 
 def test_params_and_workspace(built_lib):
-    lib = C.CDLL(built_lib)
+    lib = load(built_lib)
     P = R.params(lib)
     assert P["chunk"] % 32 == 0 and P["panel"] == 64 and P["flag_offset"] == 0
-    lib.b200spmm_coo_workspace_bytes.restype = C.c_size_t
-    lib.b200spmm_coo_workspace_bytes.argtypes = [C.c_int, C.c_int] + [C.c_int64] * 4 + [C.c_int, C.c_int, C.c_int64]
     ws = lambda *a: lib.b200spmm_coo_workspace_bytes(*a)          # noqa: E731
     small = ws(0, 0, 100, 80, 8, 1000, 1, 1, 0)
     assert small > 0 and small % 256 == 0

@@ -11,6 +11,7 @@ import textwrap
 import numpy as np
 import pytest
 
+from cudalibrarysamples_b200.lib import load
 from oracle import spmm_csr16_ref as R
 from test_abi import declared_symbols, exported
 
@@ -61,7 +62,7 @@ PATTERNS = {
 def test_walk_writes_each_entry_once(built_lib, name):
     """both walks: every row written exactly once, every entry multiplied once, pieces at the row start + multiples of P; the split
     walk writes each carry slot once and the one fix-up of a long row reads exactly its pieces' slots in ascending piece order"""
-    P = R.params(C.CDLL(built_lib))["piece"]
+    P = R.params(load(built_lib))["piece"]
     lengths = PATTERNS[name](P)
     off = np.concatenate([[0], np.cumsum(lengths)]).astype(np.int64)
     m, nnz = len(lengths), int(off[-1])
@@ -94,7 +95,7 @@ def test_walk_writes_each_entry_once(built_lib, name):
 
 
 def test_walk_spreads_a_long_row_over_many_warps(built_lib):
-    P = R.params(C.CDLL(built_lib))["piece"]
+    P = R.params(load(built_lib))["piece"]
     off = np.concatenate([[0], np.cumsum(lengths_with_a_long_row(P))])
     writes, _, pieces = R.walk(off, P)
     writers = {p[3] for p in pieces if p[0] == 2}
@@ -102,13 +103,11 @@ def test_walk_spreads_a_long_row_over_many_warps(built_lib):
 
 
 ROUTE = textwrap.dedent("""
-    import ctypes as C, sys
+    import ctypes as C, os, sys
+    sys.path.insert(0, os.path.dirname(os.path.dirname(sys.argv[1])))     # the repository: argv[1] is its built library
+    from cudalibrarysamples_b200.lib import load
     real = C.CDLL(sys.argv[2], mode=C.RTLD_GLOBAL)
-    shim = C.CDLL(sys.argv[1])
-    shim.b200spmm_csr16_route.argtypes = [C.c_void_p] * 3 + [C.c_int] * 4
-    for f in ("b200spmm_coo_route", "b200spmm_bsr_route", "b200spmm_bell_route"):
-        getattr(shim, f).argtypes = [C.c_void_p] * 3 + [C.c_int] * 4
-    shim.b200spmm_batch_count.argtypes = [C.c_void_p] * 3
+    shim = load(sys.argv[1])
     I32, I64 = 2, 3
     F32, F64, F16, BF16, C32, I8 = 0, 1, 2, 14, 4, 3
     ROW, COL = 2, 1
@@ -199,10 +198,7 @@ def test_route_table_over_real_descriptors(built_lib, mode):
 
 
 def test_host_side_argument_rejection(built_lib):
-    lib = C.CDLL(built_lib)
-    i64, vp = C.c_int64, C.c_void_p
-    lib.b200spmm_csr16.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, i64, i64, vp,
-                                   i64, C.c_int, vp, C.c_size_t]
+    lib = load(built_lib)
     one = C.c_float(1.0)
     dummy = (C.c_int * 64)()
     p = C.addressof(dummy)
@@ -225,9 +221,7 @@ def test_host_side_argument_rejection(built_lib):
 def test_workspace_bytes(built_lib):
     """the row-major copy of a K-contiguous op(B) (256-byte rounded), then two carry slots of n fp32 partial sums per chunk of P
     entries"""
-    lib = C.CDLL(built_lib)
-    lib.b200spmm_csr16_workspace_bytes.argtypes = [C.c_int64] * 5
-    lib.b200spmm_csr16_workspace_bytes.restype = C.c_size_t
+    lib = load(built_lib)
     P = R.params(lib)["piece"]
     ws = lib.b200spmm_csr16_workspace_bytes
     for k, n, nnz in ((1 << 20, 128, 16 << 20), (1000, 7, 1), (5, 256, 3 * P + 1)):
@@ -239,8 +233,7 @@ def test_workspace_bytes(built_lib):
 
 
 def test_path_selection(built_lib):
-    lib = C.CDLL(built_lib)
-    lib.b200spmm_csr16_path.argtypes = [C.c_int64, C.c_void_p, C.c_int64, C.c_int64]
+    lib = load(built_lib)
     path = lambda n=128, B=4096, sbk=128, sbj=1: lib.b200spmm_csr16_path(n, B, sbk, sbj)  # noqa: E731
     assert path() == 4 and path(n=64, sbk=64) == 2 and path(n=256, sbk=256) == 8 and path(n=129, sbk=136) == 8
     assert path(n=32, sbk=32) == 1 and path(n=1, sbk=1) == 1                          # one column per lane
@@ -251,7 +244,7 @@ def test_path_selection(built_lib):
 
 
 def test_params(built_lib):
-    P = R.params(C.CDLL(built_lib))
+    P = R.params(load(built_lib))
     assert P["piece"] >= 64 and P["lane_entries"] == 32 and P["tile_rows"] % P["warps"] == 0 and P["max_cols_per_lane"] == 8
 
 

@@ -10,6 +10,7 @@ import textwrap
 import numpy as np
 import pytest
 
+from cudalibrarysamples_b200.lib import load
 from oracle import oracle as O
 from oracle import spmm_csr_t_ref as T
 from test_abi import declared_symbols, exported
@@ -18,7 +19,6 @@ REAL = "/usr/local/cuda/lib64/libcusparse.so.12"
 NEW = ["b200spmm_csr_t", "b200spmm_csr_t_plan", "b200spmm_csr_t_layout", "b200spmm_csr_t_workspace_bytes", "b200spmm_csr_t_route",
        "b200spmv_plan_trusted"]
 F32, F64, F16, BF16 = 0, 1, 2, 14
-i64, vp = C.c_int64, C.c_void_p
 
 
 def test_header_declares_and_library_exports_the_transposed_symbols(built_lib):
@@ -67,18 +67,7 @@ def test_radix_passes():
 
 
 def _shim(built_lib):
-    lib = C.CDLL(built_lib)
-    lib.b200spmm_csr_t_layout.argtypes = [C.c_int, i64, i64, i64, i64, i64, i64, vp]
-    lib.b200spmm_csr_t_layout.restype = C.c_size_t
-    lib.b200spmm_csr_t_workspace_bytes.argtypes = [C.c_int, i64, i64, i64, i64, i64, i64]
-    lib.b200spmm_csr_t_workspace_bytes.restype = C.c_size_t
-    lib.b200spmm_csr_workspace_bytes.argtypes = [C.c_int, i64, i64, C.c_int]
-    lib.b200spmm_csr_workspace_bytes.restype = C.c_size_t
-    lib.b200spmm_csr16_workspace_bytes.argtypes = [i64] * 5
-    lib.b200spmm_csr16_workspace_bytes.restype = C.c_size_t
-    lib.b200spmm_csr_t.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, i64, i64, vp,
-                                   i64, C.c_int, C.c_int, vp, C.c_size_t]
-    lib.b200spmm_csr_t_plan.argtypes = [vp, i64, i64, i64, vp, vp, C.c_int32, vp, C.c_size_t]
+    lib = load(built_lib)
     return lib
 
 
@@ -138,11 +127,10 @@ def test_host_side_argument_rejection(built_lib):
 
 
 ROUTE = textwrap.dedent(r"""
-    import ctypes as C, sys
-    shim = C.CDLL(sys.argv[1]); real = C.CDLL(sys.argv[2])
-    shim.b200spmm_csr_t_route.argtypes = [C.c_void_p] * 3 + [C.c_int] * 4 + [C.c_void_p]
-    shim.b200spmm_csr16_route.argtypes = [C.c_void_p] * 3 + [C.c_int] * 4
-    shim.b200spmv_plan_trusted.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+    import ctypes as C, os, sys
+    sys.path.insert(0, os.path.dirname(os.path.dirname(sys.argv[1])))     # the repository: argv[1] is its built library
+    from cudalibrarysamples_b200.lib import load
+    shim = load(sys.argv[1]); real = C.CDLL(sys.argv[2])
     I32, I64 = 2, 3
     F32, F64, F16, BF16, C32 = 0, 1, 2, 14, 4
     ROW, COL = 2, 1

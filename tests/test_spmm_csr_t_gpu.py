@@ -31,14 +31,8 @@ def L():
 @pytest.fixture(scope="module")
 def N(L):
     """b200spmm_csr_ws / b200spmm_csr_workspace_bytes with 64-bit arguments, on a handle of its own"""
-    from cudalibrarysamples_b200 import build
-    n = C.CDLL(build.LIB_PATH)
-    i64, vp = C.c_int64, C.c_void_p
-    n.b200spmm_csr_ws.argtypes = [vp, C.c_int, i64, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, i64, C.c_int, vp, i64,
-                                  C.c_int, vp]
-    n.b200spmm_csr_workspace_bytes.argtypes = [C.c_int, i64, i64, C.c_int]
-    n.b200spmm_csr_workspace_bytes.restype = C.c_size_t
-    return n
+    from cudalibrarysamples_b200 import build, lib
+    return lib.load(build.LIB_PATH)
 
 
 def dev(a, dtype=None):

@@ -11,6 +11,7 @@ import textwrap
 import numpy as np
 import pytest
 
+from cudalibrarysamples_b200.lib import load
 from oracle import spmv_csr16_ref as R
 from test_abi import declared_symbols, exported
 
@@ -136,7 +137,7 @@ def patterns(E):
 
 @pytest.mark.parametrize("name", sorted(patterns(256)))
 def test_walk_properties(built_lib, name):
-    E = R.params(C.CDLL(built_lib))["chunk"]
+    E = R.params(load(built_lib))["chunk"]
     lengths = patterns(E)[name]
     off = np.concatenate([[0], np.cumsum(lengths)]).astype(np.int64)
     split_order, split_pieces = structural(off, E, True)
@@ -157,7 +158,7 @@ def route(L, fmt=CSR, op=NT, alg=DEFAULT, off=I32, col=I32, a=F16, x=None, y=Non
 
 
 def test_route_by_shape(built_lib):
-    L = C.CDLL(built_lib)
+    L = load(built_lib)
     nat = native()
     shapes = [(1 << 20, 16 << 20), (1 << 20, 4 << 20), (1 << 20, 3 << 20), (1 << 16, 1 << 20), (10 << 20, 160 << 20), (10 << 20, (160 << 20) + 5), (10 << 20, 170 << 20),
               (8192 * 8192, 5 * 8192 * 8192 - 4 * 8192), (256 ** 3, 7 * 256 ** 3 - 6 * 256 ** 2), ((1 << 20) - 1, 16 << 20)]
@@ -190,11 +191,11 @@ def test_route_by_shape(built_lib):
 
 
 ROUTE = textwrap.dedent("""
-    import ctypes as C, sys
+    import ctypes as C, os, sys
+    sys.path.insert(0, os.path.dirname(os.path.dirname(sys.argv[1])))     # the repository: argv[1] is its built library
+    from cudalibrarysamples_b200.lib import load
     real = C.CDLL(sys.argv[2], mode=C.RTLD_GLOBAL)
-    shim = C.CDLL(sys.argv[1])
-    shim.b200spmv_csr16_route.argtypes = [C.c_void_p] * 3 + [C.c_int] * 3
-    shim.b200spmv_route.argtypes = [C.c_int] * 9 + [C.c_int64] * 3
+    shim = load(sys.argv[1])
     I32, I64 = 2, 3
     F32, F64, F16, BF16, I8 = 0, 1, 2, 14, 3
     NT, TR, CT = 0, 1, 2
@@ -254,9 +255,7 @@ def test_route_over_real_descriptors(built_lib, mode):
 
 
 def test_host_side_argument_rejection(built_lib):
-    lib = C.CDLL(built_lib)
-    i64, vp = C.c_int64, C.c_void_p
-    lib.b200spmv_csr16.argtypes = [vp, C.c_int, C.c_int, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, vp, vp, C.c_size_t]
+    lib = load(built_lib)
     one = C.c_float(1.0)
     dummy = (C.c_int * 64)()
     p, o = C.addressof(dummy), C.addressof(one)
@@ -274,10 +273,7 @@ def test_host_side_argument_rejection(built_lib):
 
 
 def test_workspace_bytes_params_and_path(built_lib):
-    lib = C.CDLL(built_lib)
-    lib.b200spmv_csr16_workspace_bytes.argtypes = [C.c_int64] * 2
-    lib.b200spmv_csr16_workspace_bytes.restype = C.c_size_t
-    lib.b200spmv_csr16_path.argtypes = [C.c_void_p] * 2
+    lib = load(built_lib)
     P = R.params(lib)
     E = P["chunk"]
     assert E % 256 == 0 and P["run"] == 8 and P["warps"] >= 1

@@ -10,6 +10,7 @@ import textwrap
 import numpy as np
 import pytest
 
+from cudalibrarysamples_b200.lib import load
 from oracle import spmv_csr_z_ref as R
 from test_abi import declared_symbols, exported
 
@@ -134,7 +135,7 @@ SHAPES = [(1 << 20, 16 << 20), (10 << 20, 160 << 20), (2 << 20, 32 << 20), (8192
 
 @pytest.mark.parametrize("mode", [b"off", b"csr", b"all"])
 def test_route_table(built_lib, mode):
-    L = C.CDLL(built_lib)
+    L = load(built_lib)
     assert L.b200spmv_set_option(b"B200SPMV_GENERIC", mode) == 0
     nat = native()
     for op in (NT, TR, CT):
@@ -167,11 +168,11 @@ def test_route_table(built_lib, mode):
 
 
 ROUTE = textwrap.dedent("""
-    import ctypes as C, sys
+    import ctypes as C, os, sys
+    sys.path.insert(0, os.path.dirname(os.path.dirname(sys.argv[1])))     # the repository: argv[1] is its built library
+    from cudalibrarysamples_b200.lib import load
     real = C.CDLL(sys.argv[2], mode=C.RTLD_GLOBAL)
-    shim = C.CDLL(sys.argv[1])
-    shim.b200spmv_csr16_route.argtypes = [C.c_void_p] * 3 + [C.c_int] * 3
-    shim.b200spmv_route.argtypes = [C.c_int] * 9 + [C.c_int64] * 3
+    shim = load(sys.argv[1])
     I32, I64 = 2, 3
     F32, F64, C32, C64 = 0, 1, 4, 5
     buf = (C.c_double * 64)()
@@ -233,9 +234,7 @@ def test_route_over_real_descriptors(built_lib, mode):
 
 
 def test_host_side_argument_rejection(built_lib):
-    lib = C.CDLL(built_lib)
-    i64, vp = C.c_int64, C.c_void_p
-    lib.b200spmv_csr_z.argtypes = [vp, C.c_int, i64, i64, i64, vp, vp, vp, C.c_int32, vp, vp, C.c_int, vp, vp, vp, C.c_size_t]
+    lib = load(built_lib)
     one = (C.c_double * 2)(1.0, 0.0)
     dummy = (C.c_double * 64)()
     p, o = (C.addressof(dummy) + 15) // 16 * 16, C.addressof(one)
@@ -256,9 +255,7 @@ def test_host_side_argument_rejection(built_lib):
 
 
 def test_workspace_bytes_and_params(built_lib):
-    lib = C.CDLL(built_lib)
-    lib.b200spmv_csr_z_workspace_bytes.argtypes = [C.c_int64] * 2
-    lib.b200spmv_csr_z_workspace_bytes.restype = C.c_size_t
+    lib = load(built_lib)
     P = R.params(lib)
     E = P["chunk"]
     assert E in (128, 256) and P["run"] == 8 and P["warps"] >= 1

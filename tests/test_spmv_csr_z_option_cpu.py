@@ -6,6 +6,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from cudalibrarysamples_b200.lib import load
 from oracle import spmv_csr_z_ref as R
 
 F32, F64, F16, C32, C64 = 0, 1, 2, 4, 5
@@ -24,7 +25,7 @@ def route(L, fmt=CSR, op=0, alg=0, off=I32, col=I32, a=C64, x=None, y=None, comp
 def test_zcsr_option_switches_the_class_and_only_the_class(built_lib):
     from scripts.spmv_csr_z_bench import NATIVE
     nat = eval(NATIVE)
-    L = C.CDLL(built_lib)
+    L = load(built_lib)
     assert L.b200spmv_set_option(b"B200SPMV_ZCSR", b"sometimes") == -1
     assert L.b200spmv_set_option(b"B200SPMV_ZCSR", b"on") == 0
     try:
@@ -53,7 +54,7 @@ def test_zcsr_option_switches_the_class_and_only_the_class(built_lib):
 def test_split_walk_model_at_the_complex_chunk_size(built_lib, lengths):
     """at b200spmv_csr_z's E: every row written once, every carry slot written once and read once by one fix-up at the row's first
     chunk, and both walks add the same pieces"""
-    E = R.params(C.CDLL(built_lib))["chunk"]
+    E = R.params(load(built_lib))["chunk"]
     off = np.concatenate([[0], np.cumsum(lengths)]).astype(np.int64)
     nch = max(1, -(-int(off[-1]) // E))
     sw, sr, sp = R.walk(off, E, split=True)

@@ -12,7 +12,6 @@ from oracle import spsv_ref as R
 from test_abi import declared_symbols, exported
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, "include", "b200spsv.h")
 AXES = list(itertools.product((True, False), (False, True), (False, True)))      # lower, unit, transpose
 
 
@@ -35,10 +34,8 @@ ONE_SIDED = (5, np.array([0, 1, 2, 4, 6, 7], np.int32), np.array([0, 1, 2, 3, 0,
 
 @pytest.fixture(scope="module")
 def spsv_lib(built_lib):
-    from cudalibrarysamples_b200 import build
-    lib = ctypes.CDLL(build.SPSV_LIB_PATH)
-    lib.b200spsv_csr_workspace_bytes.restype = ctypes.c_size_t
-    return lib
+    from cudalibrarysamples_b200 import build, lib
+    return lib.load(build.SPSV_LIB_PATH, header="b200spsv.h")
 
 
 # ---------------------------------------------------------------------------------------------------- oracle
@@ -122,7 +119,7 @@ def test_route_table(spsv_lib):
 
 # ---------------------------------------------------------------------------------------------------- ABI
 def test_header_declares_the_spsv_entry_points():
-    names = declared_symbols(HEADER, "B200SPSV_EXPORT")
+    names = declared_symbols("b200spsv.h")
     for n in ["cusparseSpSV_createDescr", "cusparseSpSV_destroyDescr", "cusparseSpSV_bufferSize", "cusparseSpSV_analysis",
               "cusparseSpSV_solve", "cusparseSpSV_updateMatrix", "b200spsv_csr_workspace_bytes", "b200spsv_csr_analysis",
               "b200spsv_csr_solve", "b200spsv_csr_params", "b200spsv_csr_layout", "b200spsv_route", "b200spsv_get_stats",
@@ -133,7 +130,7 @@ def test_header_declares_the_spsv_entry_points():
 def test_spsv_library_exports_every_declared_symbol(spsv_lib):
     from cudalibrarysamples_b200 import build
     have = exported(build.SPSV_LIB_PATH)
-    assert not [n for n in declared_symbols(HEADER, "B200SPSV_EXPORT") if n not in have]
+    assert not [n for n in declared_symbols("b200spsv.h") if n not in have]
     # only SpSV from the cuSPARSE namespace: SpMV and the descriptors keep binding where they did
     assert sorted(n for n in have if n.startswith("cusparse")) == sorted(
         "cusparseSpSV_" + s for s in ("createDescr", "destroyDescr", "bufferSize", "analysis", "solve", "updateMatrix"))
