@@ -26,6 +26,9 @@ struct Config {
     int dense       = 0;    // B200SPMV_DENSE = auto|on: cusparseSparseToDense / cusparseDenseToSparse_convert.  auto (0, default):
                             //   the native kernels only in the classes measured at least at parity (DESIGN.md 3.24); on (1): every
                             //   call b200dense_route admits, so the shim's native path can be exercised before a measurement routes it
+    int banded      = 0;    // B200SPMV_BANDED = auto|on: cusparse<t>gpsvInterleavedBatch / gtsvInterleavedBatch.  auto (0, default):
+                            //   the native solves only in the classes measured at least at parity (DESIGN.md 3.25); on (1): every
+                            //   call b200banded_route admits
 };
 
 Config& config();

@@ -437,6 +437,25 @@ B200SPMV_EXPORT int b200dense2csr(void* stream, int csc, int64_t m, int64_t n, i
 B200SPMV_EXPORT int b200dense2bell(void* stream, int64_t m, int64_t n, int64_t bs, int64_t ell_cols, const void* dense, int64_t ld,
                                    int order, int value_bytes, const void* colind, void* val, int32_t base);
 
+/* Batched banded solves in the interleaved layout (batched_banded.cu; cusparse<t>gpsvInterleavedBatch / gtsvInterleavedBatch):
+ * batch independent m x m systems A_j x_j = b_j, element i of system j at i * batch + j in every array.  vtype: CUDA_R_32F,
+ * CUDA_R_64F, CUDA_C_32F or CUDA_C_64F (cudaDataType).  x holds the right-hand sides on entry and the solutions on return.  The
+ * coefficient arrays are only read, and their out-of-band slots (ds[0..1], dl[0], du[m-1], dw[m-2..m-1] of every system) never.
+ * workspace: the *_workspace_bytes() bytes, 16-byte aligned; it holds the triangular factor between the two sweeps.  One thread
+ * per system, no atomics, no host synchronisation: graph-capturable, and each solution a pure function of its system.  -1 with
+ * nothing launched on m or batch outside [1, INT32_MAX], an unknown vtype or algo, or a NULL or misaligned pointer; else the CUDA
+ * launch status.  A singular factor gives Inf / NaN in x, as a division by zero does.
+ *   b200gpsv_interleaved  pentadiagonal, row i = ds[i] x[i-2] + dl[i] x[i-1] + d[i] x[i] + du[i] x[i+1] + dw[i] x[i+2]: QR by Givens
+ *                         rotations (complex: real c, complex s), R of upper bandwidth 4.
+ *   b200gtsv_interleaved  tridiagonal, row i = dl[i] x[i-1] + d[i] x[i] + du[i] x[i+1]; algo 0: Thomas without pivoting (needs
+ *                         non-zero pivots, e.g. diagonal dominance); 1: LU with partial pivoting; 2: QR by Givens rotations. */
+B200SPMV_EXPORT int b200gpsv_interleaved(void* stream, int vtype, int64_t m, const void* ds, const void* dl, const void* d, const void* du,
+                                         const void* dw, void* x, int64_t batch, void* workspace);
+B200SPMV_EXPORT size_t b200gpsv_interleaved_workspace_bytes(int vtype, int64_t m, int64_t batch);
+B200SPMV_EXPORT int b200gtsv_interleaved(void* stream, int vtype, int algo, int64_t m, const void* dl, const void* d, const void* du, void* x,
+                                         int64_t batch, void* workspace);
+B200SPMV_EXPORT size_t b200gtsv_interleaved_workspace_bytes(int vtype, int algo, int64_t m, int64_t batch);
+
 /* The BLAS-1 part of a CG iteration, fused, all scalars in DEVICE memory (no host synchronisation, CUDA-graph capturable).
  * Replaces the cublasDdot / cublasDaxpy / cublasDnrm2 / cublasDscal calls between two cusparseSpMV calls of gpu_CG
  * (cuSPARSE/cg/cg_example.c:226-286).  fp64; vectors 16-byte aligned; `workspace` = b200cg_workspace_bytes() bytes, zeroed
@@ -615,6 +634,14 @@ B200SPMV_EXPORT int b200conv_route(int op, int64_t m, int64_t n, int64_t nnz, in
 #define B200DENSE_D2S 1
 B200SPMV_EXPORT int b200dense_route(int direction, int format, int order, int vtype, int off_type, int col_type, int base, int64_t rows,
                                     int64_t cols, int64_t nnz, int batch, int alg, int64_t bs);
+/* Where the shim sends cusparse<t>gpsvInterleavedBatch (op B200BAND_GPSV, algo 0) or cusparse<t>gtsvInterleavedBatch (op
+ * B200BAND_GTSV, algo 0 / 1 / 2): 1 = b200gpsv_interleaved / b200gtsv_interleaved, 0 = the closed library.  vtype: cudaDataType;
+ * buffer: the call's pBuffer.  Forwarded: B200SPMV_FORWARD=1, an algo outside that set, m < 3 or batch < 1 (the closed library
+ * gives its own verdict on those), a NULL or misaligned buffer, and every class not measured at least at parity with the closed
+ * library (DESIGN.md 3.25).  B200SPMV_BANDED=on makes every call this admits native.  Host logic only. */
+#define B200BAND_GPSV 0
+#define B200BAND_GTSV 1
+B200SPMV_EXPORT int b200banded_route(int op, int vtype, int algo, int64_t m, int64_t batch, const void* buffer);
 /* ---------------------------------------------------------------------------------------------- *
  * Sparse triangular solve with many right-hand sides (cusparseSpSM; cuSPARSE/spsm_csr):           *
  *   C = alpha op(T)^-1 op(B), T the selected triangle of the rows x rows CSR matrix A (int32       *
@@ -796,6 +823,45 @@ B200SPMV_EXPORT cusparseStatus_t cusparseSparseToDense(cusparseHandle_t, cuspars
                                                        cusparseSparseToDenseAlg_t, void*);
 B200SPMV_EXPORT cusparseStatus_t cusparseDenseToSparse_convert(cusparseHandle_t, cusparseConstDnMatDescr_t, cusparseSpMatDescr_t,
                                                                cusparseDenseToSparseAlg_t, void*);
+/* cusparse.h:2650-2840 -- gpsvInterleavedBatch_example.c.  bufferSizeExt returns the larger of the closed library's size and
+ * ours, so one buffer serves whichever way the solve is routed. */
+B200SPMV_EXPORT cusparseStatus_t cusparseSgtsvInterleavedBatch_bufferSizeExt(cusparseHandle_t, int, int, const float*, const float*,
+                                                                             const float*, const float*, int, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseSgtsvInterleavedBatch(cusparseHandle_t, int, int, float*, float*, float*, float*, int, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseDgtsvInterleavedBatch_bufferSizeExt(cusparseHandle_t, int, int, const double*, const double*,
+                                                                             const double*, const double*, int, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseDgtsvInterleavedBatch(cusparseHandle_t, int, int, double*, double*, double*, double*, int, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseCgtsvInterleavedBatch_bufferSizeExt(cusparseHandle_t, int, int, const cuComplex*, const cuComplex*,
+                                                                             const cuComplex*, const cuComplex*, int, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseCgtsvInterleavedBatch(cusparseHandle_t, int, int, cuComplex*, cuComplex*, cuComplex*, cuComplex*,
+                                                               int, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseZgtsvInterleavedBatch_bufferSizeExt(cusparseHandle_t, int, int, const cuDoubleComplex*,
+                                                                             const cuDoubleComplex*, const cuDoubleComplex*,
+                                                                             const cuDoubleComplex*, int, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseZgtsvInterleavedBatch(cusparseHandle_t, int, int, cuDoubleComplex*, cuDoubleComplex*,
+                                                               cuDoubleComplex*, cuDoubleComplex*, int, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseSgpsvInterleavedBatch_bufferSizeExt(cusparseHandle_t, int, int, const float*, const float*,
+                                                                             const float*, const float*, const float*, const float*, int,
+                                                                             size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseSgpsvInterleavedBatch(cusparseHandle_t, int, int, float*, float*, float*, float*, float*, float*,
+                                                               int, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseDgpsvInterleavedBatch_bufferSizeExt(cusparseHandle_t, int, int, const double*, const double*,
+                                                                             const double*, const double*, const double*, const double*,
+                                                                             int, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseDgpsvInterleavedBatch(cusparseHandle_t, int, int, double*, double*, double*, double*, double*,
+                                                               double*, int, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseCgpsvInterleavedBatch_bufferSizeExt(cusparseHandle_t, int, int, const cuComplex*, const cuComplex*,
+                                                                             const cuComplex*, const cuComplex*, const cuComplex*,
+                                                                             const cuComplex*, int, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseCgpsvInterleavedBatch(cusparseHandle_t, int, int, cuComplex*, cuComplex*, cuComplex*, cuComplex*,
+                                                               cuComplex*, cuComplex*, int, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseZgpsvInterleavedBatch_bufferSizeExt(cusparseHandle_t, int, int, const cuDoubleComplex*,
+                                                                             const cuDoubleComplex*, const cuDoubleComplex*,
+                                                                             const cuDoubleComplex*, const cuDoubleComplex*,
+                                                                             const cuDoubleComplex*, int, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseZgpsvInterleavedBatch(cusparseHandle_t, int, int, cuDoubleComplex*, cuDoubleComplex*,
+                                                               cuDoubleComplex*, cuDoubleComplex*, cuDoubleComplex*, cuDoubleComplex*, int,
+                                                               void*);
 #ifdef __cplusplus
 }
 #endif
