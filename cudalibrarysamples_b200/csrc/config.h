@@ -29,6 +29,8 @@ struct Config {
     int banded      = 0;    // B200SPMV_BANDED = auto|on: cusparse<t>gpsvInterleavedBatch / gtsvInterleavedBatch.  auto (0, default):
                             //   the native solves only in the classes measured at least at parity (DESIGN.md 3.25); on (1): every
                             //   call b200banded_route admits
+    int ilu0        = 0;    // B200SPMV_ILU0 = auto|on: cusparse<t>csrilu02 / csric02.  auto (0, default): the native factorization only
+                            //   in the classes measured at least at parity (DESIGN.md 3.26); on (1): every call b200ilu0_route admits
 };
 
 Config& config();

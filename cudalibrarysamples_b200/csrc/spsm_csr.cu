@@ -38,17 +38,6 @@ static void layout(int64_t rows, int64_t nnz, int transpose, size_t* o) {
     o[B200SPSM_TOTAL] = p;
 }
 
-// Correctly rounded operations, never contracted into an FMA: the summation order of DESIGN.md 3.20 is then a complete
-// statement of every result's bits (oracle/spsm_ref.py restates it in numpy).
-__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
-__device__ __forceinline__ double sub_rn(double a, double b) { return __dsub_rn(a, b); }
-__device__ __forceinline__ float div_rn(float a, float b) { return __fdiv_rn(a, b); }
-__device__ __forceinline__ double div_rn(double a, double b) { return __ddiv_rn(a, b); }
-
 // One warp per claimed row.  Lane = g * W + c (W = 1 << tile_log2): c picks a column of the current tile of W right-hand
 // sides, g one of 32 / W entry groups; group g sums the row's entries g, g + 32/W, ... in ascending order, and a fixed
 // xor tree over the groups adds the partial sums.  op(B)(i, j) = B[i * sbi + j * sbk], C(i, j) = C[i * sci + j * scj].
@@ -122,30 +111,6 @@ static int launch_solve(cudaStream_t s, int rows, int unit, int tile_log2, int n
         (const T*)values, (const T*)diag, on_dev ? (const T*)alpha : nullptr, on_dev ? T(0) : *(const T*)alpha, (const T*)B, sbi, sbk,
         (T*)C, sci, scj, (unsigned*)(ws + o[B200SPSM_FLAGS]), state, kSpinBudgetNs);
     return (int)cudaGetLastError();
-}
-
-// Level of every row and the level order, from the plan read back to the host: one pass in the solve direction (every
-// dependency of a row precedes it), then a stable counting sort by level.  Returns the number of levels.
-static int64_t level_order(int64_t rows, int ascending, const std::vector<int>& t_off, const std::vector<int>& t_col,
-                           std::vector<int>& order) {
-    std::vector<int> level(rows, 0);
-    int top = -1;
-    for (int64_t k = 0; k < rows; k++) {
-        const int64_t i = ascending ? k : rows - 1 - k;
-        int l = 0;
-        for (int m = t_off[i]; m < t_off[i + 1]; m++) l = std::max(l, level[t_col[m]] + 1);
-        level[i] = l;
-        top = std::max(top, l);
-    }
-    std::vector<int64_t> start(top + 2, 0);
-    for (int64_t i = 0; i < rows; i++) start[level[i] + 1]++;
-    for (int l = 0; l <= top; l++) start[l + 1] += start[l];
-    order.assign(rows, 0);
-    for (int64_t k = 0; k < rows; k++) {
-        const int64_t i = ascending ? k : rows - 1 - k;
-        order[start[level[i]]++] = (int)i;
-    }
-    return top + 1;
 }
 
 static bool flag01(int v) { return v == 0 || v == 1; }

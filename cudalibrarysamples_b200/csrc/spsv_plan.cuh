@@ -1,5 +1,5 @@
-// spsv_plan.cuh -- the triangular-solve plan and the sync-free wait protocol, shared by spsv_csr.cu (libb200spsv.so) and
-// spsm_csr.cu (libb200spmv.so).  Everything here has internal linkage: each library gets its own copy and exports none of it.
+// spsv_plan.cuh -- the triangular-solve plan, its level order and the sync-free wait protocol, shared by spsv_csr.cu
+// (libb200spsv.so), spsm_csr.cu and ilu0_csr.cu (libb200spmv.so).  Nothing here is exported: each library gets its own copy.
 //
 // The plan of op(A)'s selected triangle: t_off / t_col / t_vidx, the triangle without its diagonal as CSR whose entries point
 // back into the caller's values, and diag_vidx, the diagonal's index per row (include/b200spsv.h has the layout).
@@ -9,6 +9,7 @@
 
 #include <algorithm>
 #include <cstdint>
+#include <vector>
 
 #include "spmv_common.cuh"
 
@@ -20,6 +21,17 @@ constexpr uint64_t kSpinBudgetNs = 4000000000ull;         // 4 s per wait: far b
 enum { ST_EPOCH = 0, ST_CLAIM = 1, ST_ERROR = 2, ST_MISSING = 3 };
 
 using b200::round_up_256;
+
+// Correctly rounded operations, never contracted into an FMA: a summation order is then a complete statement of every result's
+// bits (oracle/spsm_ref.py and oracle/ilu0_ref.py restate them in numpy).
+__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
+__device__ __forceinline__ double sub_rn(double a, double b) { return __dsub_rn(a, b); }
+__device__ __forceinline__ float div_rn(float a, float b) { return __fdiv_rn(a, b); }
+__device__ __forceinline__ double div_rn(double a, double b) { return __ddiv_rn(a, b); }
 
 // ------------------------------------------------------------------------------------------------ analysis
 // Per row r of A: the first stored diagonal (NON_UNIT), and the number of selected off-diagonal entries -- of row r of
@@ -145,6 +157,32 @@ static cudaError_t build_plan(cudaStream_t s, int64_t rows, int64_t nnz, const i
         if (err != cudaSuccess) return err;
     }
     return cudaGetLastError();
+}
+
+// Level of every row and the level order, from the plan read back to the host: one pass in the solve direction (every
+// dependency of a row precedes it), then a stable counting sort by level.  Returns the number of levels; level_start, when
+// not NULL, receives where each level begins in order[] (levels + 1 entries, the last == rows).
+static int64_t level_order(int64_t rows, int ascending, const std::vector<int>& t_off, const std::vector<int>& t_col,
+                           std::vector<int>& order, std::vector<int>* level_start = nullptr) {
+    std::vector<int> level(rows, 0);
+    int top = -1;
+    for (int64_t k = 0; k < rows; k++) {
+        const int64_t i = ascending ? k : rows - 1 - k;
+        int l = 0;
+        for (int m = t_off[i]; m < t_off[i + 1]; m++) l = std::max(l, level[t_col[m]] + 1);
+        level[i] = l;
+        top = std::max(top, l);
+    }
+    std::vector<int64_t> start(top + 2, 0);
+    for (int64_t i = 0; i < rows; i++) start[level[i] + 1]++;
+    for (int l = 0; l <= top; l++) start[l + 1] += start[l];
+    if (level_start) level_start->assign(start.begin(), start.end());
+    order.assign(rows, 0);
+    for (int64_t k = 0; k < rows; k++) {
+        const int64_t i = ascending ? k : rows - 1 - k;
+        order[start[level[i]]++] = (int)i;
+    }
+    return top + 1;
 }
 
 // ------------------------------------------------------------------------------------------------ solve protocol

@@ -539,6 +539,8 @@ B200SPMV_EXPORT int b200spmv_sell_generic_mv(void* stream, int off64, int col64,
  *                      COO, Sliced-ELL and strided-batch SpMM, which have not had their first hardware run yet)
  *   B200SPMV_ZCSR = auto|on (cusparseSpMV on a double-complex CSR A: auto [default] = b200spmv_csr_z only in the classes measured at
  *                      least at parity with the closed library (none today, DESIGN.md 3.21); on = every call in its class)
+ *   B200SPMV_DENSE / B200SPMV_BANDED / B200SPMV_ILU0 = auto|on (the same choice for the conversions, the batched banded solves and
+ *                      cusparse<t>csrilu02 / csric02)
  * returns 0, or -1 for an unknown key / value. */
 B200SPMV_EXPORT int  b200spmv_set_option(const char* key, const char* value);
 /* Call counters of the cuSPARSE-symbol layer: SpMV calls that ran on our kernels, SpMV calls handed to the closed library
@@ -691,6 +693,66 @@ B200SPMV_EXPORT int b200spsm_route(int format, int opA, int opB, int alg, int of
 /* Since the last reset: SpSM solves run natively / SpSM calls handed to the closed library / native analyses. */
 B200SPMV_EXPORT void b200spsm_get_stats(uint64_t* native_calls, uint64_t* forwarded_calls, uint64_t* analysis_calls);
 B200SPMV_EXPORT void b200spsm_reset_stats(void);
+/* ---------------------------------------------------------------------------------------------- *
+ * Incomplete LU and Cholesky factorization without fill-in (cusparse<t>csrilu02 / csric02;       *
+ * cuSPARSE/bicgstab, cuSPARSE/cg), ilu0_csr.cu:                                                  *
+ *   the rows x rows CSR matrix A (int32 offsets and columns, index base 0 or 1, columns strictly  *
+ *   ascending in every row) is overwritten in place by its factor.  A row without a stored        *
+ *   diagonal is a structural zero: it is left as stored, and nothing is read from it.             *
+ *   kind B200ILU0_LU: row i becomes L (unit, strictly lower) and U (upper with the diagonal).      *
+ *   kind B200ILU0_IC: the lower triangle with the diagonal becomes L (A ~ L L^T); entries with     *
+ *   column > row are never read or written.  dtype 0 = fp32, 1 = fp64.  Every operation is one    *
+ *   correctly rounded mul / sub / div / sqrt, each entry a left fold in ascending column order    *
+ *   (DESIGN.md 3.26): the bits are the plain sequential algorithm's, whatever the schedule.        *
+ *   return: 0, -1 on invalid arguments (checked before any CUDA call), else the cudaError_t.      *
+ * ---------------------------------------------------------------------------------------------- */
+#define B200ILU0_LU 0
+#define B200ILU0_IC 1
+#define B200ILU0_BAD_PATTERN (-2)       /* analysis: a row with unsorted, duplicate or out-of-range columns, or offsets that decrease
+                                           or leave [base, nnz + base] */
+#define B200ILU0_NO_COOPERATIVE (-3)    /* analysis: the current device cannot launch cooperative kernels */
+/* Bytes of the workspace analysis builds the schedule in; pass it to every factorization and zero-pivot query of that pattern. */
+B200SPMV_EXPORT size_t b200ilu0_workspace_bytes(int64_t rows, int64_t nnz);
+/* Byte offsets of the workspace's arrays, each 256-byte aligned: the state words (uint32: [4] levels, [5] zero-pivot row,
+ * [6] rows with a bad pattern, [7] first row without a stored diagonal; INT32_MAX for "none"), diag[rows] (position of each
+ * row's diagonal), order[rows] (rows by level, ascending within a level), level_start[rows + 1], then what only analysis uses:
+ * SpSV's strictly-lower plan t_off / t_col / t_vidx, the offsets clamped to [base, nnz + base] and scratch.
+ * offsets[B200ILU0_TOTAL] == b200ilu0_workspace_bytes(...).
+ * Returns -1 for negative sizes. */
+enum { B200ILU0_STATE = 0, B200ILU0_DIAG, B200ILU0_ORDER, B200ILU0_LEVEL_START, B200ILU0_T_OFF, B200ILU0_T_COL, B200ILU0_T_VIDX,
+       B200ILU0_CHECKED_OFF, B200ILU0_SCRATCH, B200ILU0_TOTAL, B200ILU0_LAYOUT_N };
+B200SPMV_EXPORT int b200ilu0_layout(int64_t rows, int64_t nnz, size_t* offsets /* [B200ILU0_LAYOUT_N] */);
+/* Checks the pattern, finds each row's diagonal and the level schedule of the strictly-lower dependency graph (integer work;
+ * values are not read).  The offsets are checked and clamped first, so no kernel indexes col_ind outside [0, nnz).  Synchronises
+ * the stream once: the levels are computed on the host.  structural_zero receives the first
+ * row without a stored diagonal, or -1; levels the number of levels.  Returns B200ILU0_BAD_PATTERN or B200ILU0_NO_COOPERATIVE
+ * (nothing else in the workspace is then valid) as above. */
+B200SPMV_EXPORT int b200ilu0_analysis(void* stream, int64_t rows, int64_t nnz, const void* row_offsets, const void* col_ind, int32_t base,
+                                      void* workspace, int64_t* structural_zero, int64_t* levels);
+/* Factorizes values in place on the schedule analysis built: one cooperative launch, warps take the rows of a level by static
+ * striding, a grid-wide barrier between levels.  LU: with boost = 1, a pivot with |a_ii| <= *tol becomes *boost_val after its
+ * row's updates.  tol (one double) and boost_val (one value of dtype) are host pointers, or device pointers read by the kernel
+ * (on_device = 1); unused when boost = 0.  The zero-pivot word receives the smallest row whose pivot is zero (LU, after the
+ * boost) or not positive (IC, before its square root), or the structural zero analysis found when that is smaller.  Rows without
+ * a stored diagonal are left as stored, and a step whose row k has none is skipped: the factor is then defined, not meaningful.
+ * No allocation, no host synchronisation. */
+B200SPMV_EXPORT int b200ilu0_factor(void* stream, int kind, int dtype, int64_t rows, int64_t nnz, const void* row_offsets,
+                                    const void* col_ind, int32_t base, void* values, int boost, const void* tol, const void* boost_val,
+                                    int on_device, void* workspace);
+/* The smallest row with a structural zero (analysis) or a zero pivot (the latest factorization), -1 for none, as
+ * cusparseXcsrilu02_zeroPivot reports it: into the host int32 at position (on_device = 0), or by a kernel into the device int32 at
+ * position (on_device = 1).  Synchronises the stream either way, as the closed call does, and writes the row to the host int64 at
+ * row when not NULL. */
+B200SPMV_EXPORT int b200ilu0_zero_pivot(void* stream, const void* workspace, void* position, int on_device, int64_t* row);
+/* Threads per CTA of the factorization kernel and the CTAs per SM it launches at most. */
+B200SPMV_EXPORT void b200ilu0_params(int32_t* threads_per_cta, int32_t* ctas_per_sm);
+/* Where the shim's cusparse<t>csrilu02 / csric02 analysis sends a pattern (kind B200ILU0_LU / _IC, vtype: cudaDataType,
+ * levels: b200ilu0_analysis' count): 1 = b200ilu0_factor, 0 = the closed library.  levels = 0 asks before analysis: 1 when some
+ * level count could be native.  The shim asks that first, and where the answer is 0 (every call in the default mode today) its
+ * bufferSize and analysis are the closed library's alone, with no native work.  Forwarded: B200SPMV_FORWARD=1, types other than
+ * CUDA_R_32F / CUDA_R_64F, sizes outside int32, and every class not measured at least at parity with the closed library
+ * (DESIGN.md 3.26).  B200SPMV_ILU0=on makes every call this admits native.  Host logic only. */
+B200SPMV_EXPORT int b200ilu0_route(int kind, int vtype, int64_t rows, int64_t nnz, int64_t levels);
 /* name of the main kernel the most recent CSR SpMV launched, e.g. "b200::csr_seg_kernel<double>" (bench.py's roofline.kernel) */
 B200SPMV_EXPORT const char* b200spmv_last_csr_kernel(void);
 
@@ -862,6 +924,83 @@ B200SPMV_EXPORT cusparseStatus_t cusparseZgpsvInterleavedBatch_bufferSizeExt(cus
 B200SPMV_EXPORT cusparseStatus_t cusparseZgpsvInterleavedBatch(cusparseHandle_t, int, int, cuDoubleComplex*, cuDoubleComplex*,
                                                                cuDoubleComplex*, cuDoubleComplex*, cuDoubleComplex*, cuDoubleComplex*, int,
                                                                void*);
+/* cusparse.h:434-454, 1434-1666, 1942-2100 -- cg_example.c:423-458, bicgstab_example.c:511-543.  Info objects stay real; the shim
+ * keeps a side-table entry per info.  bufferSize returns the larger of the closed library's size and ours; C and Z forward.  The
+ * closed library declares the _bufferSizeExt variants but does not export them: the shim's take its _bufferSize and widen it. */
+B200SPMV_EXPORT cusparseStatus_t cusparseCreateCsrilu02Info(csrilu02Info_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseDestroyCsrilu02Info(csrilu02Info_t);
+B200SPMV_EXPORT cusparseStatus_t cusparseCreateCsric02Info(csric02Info_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseDestroyCsric02Info(csric02Info_t);
+B200SPMV_EXPORT cusparseStatus_t cusparseXcsrilu02_zeroPivot(cusparseHandle_t, csrilu02Info_t, int*);
+B200SPMV_EXPORT cusparseStatus_t cusparseXcsric02_zeroPivot(cusparseHandle_t, csric02Info_t, int*);
+B200SPMV_EXPORT cusparseStatus_t cusparseScsrilu02_numericBoost(cusparseHandle_t, csrilu02Info_t, int, double*, float*);
+B200SPMV_EXPORT cusparseStatus_t cusparseDcsrilu02_numericBoost(cusparseHandle_t, csrilu02Info_t, int, double*, double*);
+B200SPMV_EXPORT cusparseStatus_t cusparseCcsrilu02_numericBoost(cusparseHandle_t, csrilu02Info_t, int, double*, cuComplex*);
+B200SPMV_EXPORT cusparseStatus_t cusparseZcsrilu02_numericBoost(cusparseHandle_t, csrilu02Info_t, int, double*, cuDoubleComplex*);
+B200SPMV_EXPORT cusparseStatus_t cusparseScsrilu02_bufferSize(cusparseHandle_t, int, int, const cusparseMatDescr_t, float*, const int*,
+                                                              const int*, csrilu02Info_t, int*);
+B200SPMV_EXPORT cusparseStatus_t cusparseDcsrilu02_bufferSize(cusparseHandle_t, int, int, const cusparseMatDescr_t, double*, const int*,
+                                                              const int*, csrilu02Info_t, int*);
+B200SPMV_EXPORT cusparseStatus_t cusparseCcsrilu02_bufferSize(cusparseHandle_t, int, int, const cusparseMatDescr_t, cuComplex*,
+                                                              const int*, const int*, csrilu02Info_t, int*);
+B200SPMV_EXPORT cusparseStatus_t cusparseZcsrilu02_bufferSize(cusparseHandle_t, int, int, const cusparseMatDescr_t, cuDoubleComplex*,
+                                                              const int*, const int*, csrilu02Info_t, int*);
+B200SPMV_EXPORT cusparseStatus_t cusparseScsrilu02_bufferSizeExt(cusparseHandle_t, int, int, const cusparseMatDescr_t, float*,
+                                                                 const int*, const int*, csrilu02Info_t, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseDcsrilu02_bufferSizeExt(cusparseHandle_t, int, int, const cusparseMatDescr_t, double*,
+                                                                 const int*, const int*, csrilu02Info_t, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseCcsrilu02_bufferSizeExt(cusparseHandle_t, int, int, const cusparseMatDescr_t, cuComplex*,
+                                                                 const int*, const int*, csrilu02Info_t, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseZcsrilu02_bufferSizeExt(cusparseHandle_t, int, int, const cusparseMatDescr_t, cuDoubleComplex*,
+                                                                 const int*, const int*, csrilu02Info_t, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseScsrilu02_analysis(cusparseHandle_t, int, int, const cusparseMatDescr_t, const float*,
+                                                            const int*, const int*, csrilu02Info_t, cusparseSolvePolicy_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseDcsrilu02_analysis(cusparseHandle_t, int, int, const cusparseMatDescr_t, const double*,
+                                                            const int*, const int*, csrilu02Info_t, cusparseSolvePolicy_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseCcsrilu02_analysis(cusparseHandle_t, int, int, const cusparseMatDescr_t, const cuComplex*,
+                                                            const int*, const int*, csrilu02Info_t, cusparseSolvePolicy_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseZcsrilu02_analysis(cusparseHandle_t, int, int, const cusparseMatDescr_t, const cuDoubleComplex*,
+                                                            const int*, const int*, csrilu02Info_t, cusparseSolvePolicy_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseScsrilu02(cusparseHandle_t, int, int, const cusparseMatDescr_t, float*, const int*, const int*,
+                                                   csrilu02Info_t, cusparseSolvePolicy_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseDcsrilu02(cusparseHandle_t, int, int, const cusparseMatDescr_t, double*, const int*, const int*,
+                                                   csrilu02Info_t, cusparseSolvePolicy_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseCcsrilu02(cusparseHandle_t, int, int, const cusparseMatDescr_t, cuComplex*, const int*,
+                                                   const int*, csrilu02Info_t, cusparseSolvePolicy_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseZcsrilu02(cusparseHandle_t, int, int, const cusparseMatDescr_t, cuDoubleComplex*, const int*,
+                                                   const int*, csrilu02Info_t, cusparseSolvePolicy_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseScsric02_bufferSize(cusparseHandle_t, int, int, const cusparseMatDescr_t, float*, const int*,
+                                                             const int*, csric02Info_t, int*);
+B200SPMV_EXPORT cusparseStatus_t cusparseDcsric02_bufferSize(cusparseHandle_t, int, int, const cusparseMatDescr_t, double*, const int*,
+                                                             const int*, csric02Info_t, int*);
+B200SPMV_EXPORT cusparseStatus_t cusparseCcsric02_bufferSize(cusparseHandle_t, int, int, const cusparseMatDescr_t, cuComplex*,
+                                                             const int*, const int*, csric02Info_t, int*);
+B200SPMV_EXPORT cusparseStatus_t cusparseZcsric02_bufferSize(cusparseHandle_t, int, int, const cusparseMatDescr_t, cuDoubleComplex*,
+                                                             const int*, const int*, csric02Info_t, int*);
+B200SPMV_EXPORT cusparseStatus_t cusparseScsric02_bufferSizeExt(cusparseHandle_t, int, int, const cusparseMatDescr_t, float*,
+                                                                const int*, const int*, csric02Info_t, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseDcsric02_bufferSizeExt(cusparseHandle_t, int, int, const cusparseMatDescr_t, double*,
+                                                                const int*, const int*, csric02Info_t, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseCcsric02_bufferSizeExt(cusparseHandle_t, int, int, const cusparseMatDescr_t, cuComplex*,
+                                                                const int*, const int*, csric02Info_t, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseZcsric02_bufferSizeExt(cusparseHandle_t, int, int, const cusparseMatDescr_t, cuDoubleComplex*,
+                                                                const int*, const int*, csric02Info_t, size_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseScsric02_analysis(cusparseHandle_t, int, int, const cusparseMatDescr_t, const float*,
+                                                           const int*, const int*, csric02Info_t, cusparseSolvePolicy_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseDcsric02_analysis(cusparseHandle_t, int, int, const cusparseMatDescr_t, const double*,
+                                                           const int*, const int*, csric02Info_t, cusparseSolvePolicy_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseCcsric02_analysis(cusparseHandle_t, int, int, const cusparseMatDescr_t, const cuComplex*,
+                                                           const int*, const int*, csric02Info_t, cusparseSolvePolicy_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseZcsric02_analysis(cusparseHandle_t, int, int, const cusparseMatDescr_t, const cuDoubleComplex*,
+                                                           const int*, const int*, csric02Info_t, cusparseSolvePolicy_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseScsric02(cusparseHandle_t, int, int, const cusparseMatDescr_t, float*, const int*, const int*,
+                                                  csric02Info_t, cusparseSolvePolicy_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseDcsric02(cusparseHandle_t, int, int, const cusparseMatDescr_t, double*, const int*, const int*,
+                                                  csric02Info_t, cusparseSolvePolicy_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseCcsric02(cusparseHandle_t, int, int, const cusparseMatDescr_t, cuComplex*, const int*,
+                                                  const int*, csric02Info_t, cusparseSolvePolicy_t, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseZcsric02(cusparseHandle_t, int, int, const cusparseMatDescr_t, cuDoubleComplex*, const int*,
+                                                  const int*, csric02Info_t, cusparseSolvePolicy_t, void*);
 #ifdef __cplusplus
 }
 #endif
