@@ -11,10 +11,31 @@ sm_90a operator.  Vector updates and dot products are torch ops (plumbing); the 
 """
 from __future__ import annotations
 
+import contextlib
+
 import torch
 import torch.distributed as dist
 
 from .sharded import ShardedCsr
+
+
+@contextlib.contextmanager
+def side_stream(sh: ShardedCsr):
+    """A fresh stream for CUDA-graph capture (capture needs a stream other than the default one), made current, with the
+    library handles of the sharded operator moved onto it; on exit the handles go back and the caller's stream waits for it."""
+    main = torch.cuda.current_stream()
+    side = torch.cuda.Stream()
+    side.wait_stream(main)
+    ops = [op for op in (getattr(sh, "local_op", None), getattr(sh, "own_op", None)) if op is not None and hasattr(op, "handle")]
+    try:
+        with torch.cuda.stream(side):
+            for op in ops:
+                op.api.cusparseSetStream(op.handle, side.cuda_stream)
+            yield side
+    finally:
+        main.wait_stream(side)
+        for op in ops:
+            op.api.cusparseSetStream(op.handle, main.cuda_stream)
 
 
 def _dot(a: torch.Tensor, b: torch.Tensor, world: int, group=None) -> torch.Tensor:
@@ -151,13 +172,7 @@ class FusedCgSolver:
         return x, [float(v) for v in norms.tolist()]
 
     def _run_graphed(self, x, r, p, t, iters):
-        main = torch.cuda.current_stream()
-        side = torch.cuda.Stream()
-        side.wait_stream(main)
-        ops = [op for op in (getattr(self.sh, "local_op", None), getattr(self.sh, "own_op", None)) if op is not None and hasattr(op, "handle")]
-        with torch.cuda.stream(side):
-            for op in ops:
-                op.api.cusparseSetStream(op.handle, side.cuda_stream)
+        with side_stream(self.sh) as side:
             self._iteration(x, r, p, t, 0)            # two eager iterations: warm-up of every kernel on this stream
             self._iteration(x, r, p, t, 1)
             g = torch.cuda.CUDAGraph()
@@ -169,9 +184,6 @@ class FusedCgSolver:
             while done + 2 <= iters:
                 g.replay()
                 done += 2
-        main.wait_stream(side)
-        for op in ops:
-            op.api.cusparseSetStream(op.handle, main.cuda_stream)
         self._graph = g
         return done
 

@@ -16,41 +16,10 @@
 // order.  fp64 only (the solvers of the reference are fp64: cg_example.c:311, bicgstab_example.c:375).
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include "spmv_common.cuh"
+#include "cg_reduce.cuh"
 #include "../../include/b200spmv.h"
 
 namespace b200cg {
-
-constexpr int BLOCK = 256;
-constexpr int MAX_CTAS = 132 * 16;   // 256 threads x 16 CTAs/SM candidates: plenty of loads in flight for a pure stream
-
-// workspace: [0 .. MAX_CTAS) partial sums, then one arrival counter (as a double slot)
-__device__ __forceinline__ double block_sum(double v, double* sred) {
-    v = b200::warp_allsum(v);
-    if ((threadIdx.x & 31) == 0) sred[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double t = 0;
-    if (threadIdx.x == 0) {
-#pragma unroll
-        for (int w = 0; w < BLOCK / 32; w++) t += sred[w];
-    }
-    return t;      // valid on thread 0
-}
-
-// thread 0 of every CTA calls this with its CTA's partial; the last CTA to arrive writes the total (fixed CTA order)
-__device__ __forceinline__ void grid_sum_finish(double part, double* ws, double* out) {
-    unsigned* counter = (unsigned*)(ws + MAX_CTAS);
-    ws[blockIdx.x] = part;
-    __threadfence();
-    const unsigned arrived = atomicAdd(counter, 1u);
-    if (arrived == gridDim.x - 1) {
-        __threadfence();
-        double t = 0;
-        for (unsigned b = 0; b < gridDim.x; b++) t += __ldcg(ws + b);
-        *out = t;
-        *counter = 0u;
-    }
-}
 
 __global__ void __launch_bounds__(BLOCK) dot_kernel(int64_t n, const double* __restrict__ a, const double* __restrict__ b,
                                                     double* __restrict__ out, double* __restrict__ ws) {
@@ -161,14 +130,6 @@ __global__ void __launch_bounds__(BLOCK) update_xp_kernel(int64_t n, double* __r
         }
     }
 }
-
-static int grid_for(int64_t n) {
-    int64_t g = (n / 2 + BLOCK - 1) / BLOCK;
-    if (g > MAX_CTAS) g = MAX_CTAS;
-    if (g < 1) g = 1;
-    return (int)g;
-}
-static bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 
 }  // namespace b200cg
 

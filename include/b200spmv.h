@@ -483,6 +483,62 @@ B200SPMV_EXPORT int    b200cg_update_xp(void* stream, int64_t n, double* x, doub
 B200SPMV_EXPORT int    b200cg_update_p(void* stream, int64_t n, double* p, const double* r, const double* delta_new,
                                        const double* delta);
 
+/* The BLAS-1 part of an unpreconditioned BiCGStab iteration (cuSPARSE/bicgstab/bicgstab_example.c:212-351 with M = I), fused,
+ * with every scalar AND every decision (convergence, breakdown) in device memory: no host synchronisation, CUDA-graph
+ * capturable.  fp64; vectors 16-byte aligned; same walk, grid and deterministic reduction as b200cg_* (b200cg_params).
+ * `workspace` = b200bicgstab_workspace_bytes() bytes, zeroed once by the caller; it also serves b200cg_dot (the arrival
+ * counter sits at the same byte, max_ctas * 8, and every reduction leaves it at zero).
+ * `state`: 16-byte aligned, b200bicgstab_state_layout(history_len) bytes: doubles at the B200BICGSTAB_* slot indices below,
+ * then the int32 status, the int32 count of finished iterations, and history_len doubles of ||r|| (entry k after iteration
+ * k, entry 0 = ||r0||; entries past history_len are not recorded).  The layout call reports the byte offsets.
+ * One iteration, after r0 = b - A x0 and b200cg_dot(r0, r0 -> state[RHO_NEW]) then b200bicgstab_init:
+ *   v = A p;  b200cg_dot(r0, v -> state[DENOM])
+ *   b200bicgstab_update_s   alpha = rho_new / denom;  s = r - alpha v;  s2 = s . s;  rho <- rho_new
+ *   t = A s;  b200bicgstab_dot2   ts = t . s,  tt = t . t
+ *   b200bicgstab_update_xr  sqrt(s2) < threshold: x += alpha p, r = s, status CONVERGED_S;
+ *                           else omega = ts / tt, x += alpha p + omega s, r = s - omega t;  then rho_new = r0 . r, r2 = r . r
+ *   b200bicgstab_update_p   sqrt(r2) < threshold: status CONVERGED_R;
+ *                           else beta = (rho_new / rho) (alpha / omega), p = r + beta (p - omega v)
+ * A caller on several ranks all-reduces (sum) state[DENOM], then state[S2 .. TT] (contiguous), then state[RHO_NEW .. R2]
+ * (contiguous) after the call that produced them; every decision is taken at kernel entry from those reduced values, so all
+ * ranks stop at the same iteration.  A breakdown (denom = 0, tt = 0, omega = 0, rho_new = 0, or a non-finite scalar) sets its
+ * status and updates nothing, so x never holds a NaN.  Once the status is not RUNNING every b200bicgstab_* iteration call
+ * returns at entry: x, r, p and the state stay bit-identical (b200cg_dot still writes denom).  tol < 0: no convergence test.
+ * Each call returns -1 with nothing launched on n < 0, a NULL or misaligned pointer (vectors may be NULL when n = 0), a
+ * history_len outside [0, INT32_MAX] or a NaN tol; else the CUDA launch status. */
+#define B200BICGSTAB_RHO        0      /* rho_{k-1}: r0 . r before this iteration */
+#define B200BICGSTAB_ALPHA      1
+#define B200BICGSTAB_OMEGA      2
+#define B200BICGSTAB_DENOM      3      /* r0 . v */
+#define B200BICGSTAB_S2         4      /* s . s   \                                        */
+#define B200BICGSTAB_TS         5      /* t . s    | reduced (and all-reduced) together    */
+#define B200BICGSTAB_TT         6      /* t . t   /                                        */
+#define B200BICGSTAB_RHO_NEW    7      /* r0 . r  \ reduced together                       */
+#define B200BICGSTAB_R2         8      /* r . r   /                                        */
+#define B200BICGSTAB_THRESHOLD  9      /* tol * ||r0||, or -1 when there is no convergence test */
+#define B200BICGSTAB_RUNNING             0
+#define B200BICGSTAB_CONVERGED_S         1
+#define B200BICGSTAB_CONVERGED_R         2
+#define B200BICGSTAB_BREAKDOWN_DENOM     3
+#define B200BICGSTAB_BREAKDOWN_TT        4
+#define B200BICGSTAB_BREAKDOWN_OMEGA     5
+#define B200BICGSTAB_BREAKDOWN_RHO       6
+#define B200BICGSTAB_BREAKDOWN_NONFINITE 7
+B200SPMV_EXPORT size_t b200bicgstab_workspace_bytes(void);
+/* the state block's size in bytes for history_len history entries (0 when history_len is outside [0, INT32_MAX]); the byte
+ * offsets of the status, the iteration counter and the history go to the non-NULL pointers */
+B200SPMV_EXPORT size_t b200bicgstab_state_layout(int64_t history_len, int32_t* status_byte, int32_t* iter_byte, int32_t* history_byte);
+/* r = p = r0;  rho = r2 = state[RHO_NEW];  threshold = tol * sqrt(rho);  counter 0;  history[0] = sqrt(rho);  status RUNNING,
+ * CONVERGED_R when rho = 0 (x0 solves the system), BREAKDOWN_NONFINITE when rho is not finite */
+B200SPMV_EXPORT int    b200bicgstab_init(void* stream, int64_t n, const double* r0, double* r, double* p, void* state,
+                                         int64_t history_len, double tol);
+B200SPMV_EXPORT int    b200bicgstab_update_s(void* stream, int64_t n, const double* r, const double* v, double* s, void* state,
+                                             void* workspace);
+B200SPMV_EXPORT int    b200bicgstab_dot2(void* stream, int64_t n, const double* t, const double* s, void* state, void* workspace);
+B200SPMV_EXPORT int    b200bicgstab_update_xr(void* stream, int64_t n, double* x, double* r, const double* p, const double* s,
+                                              const double* t, const double* r0, void* state, void* workspace);
+B200SPMV_EXPORT int    b200bicgstab_update_p(void* stream, int64_t n, double* p, const double* r, const double* v, void* state);
+
 /* Device-side barrier over NVLink peer memory (one process per GPU, one box), graph-replay safe: the epoch lives in device
  * memory.  peer_flag_ptrs_dev: device array of `world` pointers, entry r = rank r's flag array (`world` 8-byte slots,
  * zero-initialised, mapped into this process: symmetric memory / CUDA IPC); epoch_dev: one zero-initialised 8-byte counter
