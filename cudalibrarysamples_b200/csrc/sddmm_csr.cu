@@ -134,12 +134,11 @@ static SddmmCopies sddmm_copies(int dtype, int64_t m, int64_t n, int64_t k, int6
                                 int64_t a_stride, int64_t b_stride) {
     SddmmCopies c;
     const size_t vsz = dtype == 1 ? 8 : 4;
-    const int64_t kmax = 32LL * 65535;                           // grid.y of spmm_transpose_b_kernel
-    if (k > 1 && k <= kmax && sak != 1 && sai == 1 && m > 0) {
+    if (k > 1 && sak != 1 && sai == 1 && m > 0) {
         c.a = true;
         c.a_bytes = round_up_256((size_t)(batch > 1 && a_stride != 0 ? batch : 1) * (size_t)m * (size_t)k * vsz);
     }
-    if (k > 1 && k <= kmax && sbk != 1 && sbj == 1 && n > 0) {
+    if (k > 1 && sbk != 1 && sbj == 1 && n > 0) {
         c.b = true;
         c.b_bytes = round_up_256((size_t)(batch > 1 && b_stride != 0 ? batch : 1) * (size_t)n * (size_t)k * vsz);
     }

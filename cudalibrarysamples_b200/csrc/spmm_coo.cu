@@ -265,7 +265,7 @@ static CooMmLayout coo_mm_layout(int dtype, int64_t kdim, int64_t n, int64_t nnz
     CooMmLayout l;
     const size_t vsz = dtype == 1 ? 8 : 4;
     const double nchunks = (double)((nnz + COO_MM_CHUNK - 1) / COO_MM_CHUNK), npanels = (double)((n + COO_MM_PANEL - 1) / COO_MM_PANEL);
-    l.copy_b = !b_row_major && n >= COO_MM_MIN_N_FOR_TRANSPOSE && kdim > 0 && nnz > 0 && n <= 32LL * 65535;
+    l.copy_b = !b_row_major && n >= COO_MM_MIN_N_FOR_TRANSPOSE && kdim > 0 && nnz > 0;
     const double nb = b_stride != 0 && batch > 1 ? batch : 1;
     const double est = 4.0 * batch + 8.0 * batch * nchunks + (double)vsz * batch * nchunks * npanels * 2 * COO_MM_PANEL +
                        (l.copy_b ? (double)vsz * nb * kdim * n : 0.0) + 1024.0;

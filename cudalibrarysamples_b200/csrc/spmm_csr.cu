@@ -119,9 +119,10 @@ __global__ void __launch_bounds__(32 * SPMM_WARPS) spmm_csr_ctile_kernel(const S
     }
 }
 
-// The transpose of spmm_transpose_b_kernel (spmv_common.cuh) as a host call on `stream` (dtype 0 = fp32, 1 = fp64): sddmm_csr.cu uses it to make an operand K-contiguous.
+// The transpose of spmm_transpose_b_kernel (spmv_common.cuh) as a host call on `stream` (dtype 0 = fp32, 1 = fp64): launch_spmm below
+// makes its row-major copy of B with it, spmm_coo.cu likewise, and sddmm_csr.cu makes an operand K-contiguous.
 int transpose_col_to_row_major(cudaStream_t stream, int dtype, const void* B, int64_t ldb, void* Bt, int64_t cols, int64_t n) {
-    const dim3 tg((unsigned)((cols + 31) / 32), (unsigned)((n + 31) / 32));
+    const dim3 tg = spmm_transpose_b_grid(cols, n);
     if (dtype == 1) spmm_transpose_b_kernel<double><<<tg, 256, 0, stream>>>((const double*)B, (long long)ldb, (double*)Bt, (int)cols, (int)n);
     else spmm_transpose_b_kernel<float><<<tg, 256, 0, stream>>>((const float*)B, (long long)ldb, (float*)Bt, (int)cols, (int)n);
     return (int)cudaGetLastError();
@@ -138,10 +139,8 @@ static int launch_spmm(cudaStream_t stream, int64_t rows, int64_t n, const void*
     a.base = base; a.rows = (int)rows; a.n = (int)n;
     if (!b_row_major && workspace && n >= SPMM_MIN_N_FOR_TRANSPOSE && cols > 0) {
         // the sample's layout: one pass turns B into a row-major copy in the caller's buffer
-        const dim3 tg((unsigned)((cols + 31) / 32), (unsigned)((n + 31) / 32));
-        spmm_transpose_b_kernel<T><<<tg, 256, 0, stream>>>((const T*)B, (long long)ldb, (T*)workspace, (int)cols, (int)n);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return (int)e;
+        const int e = transpose_col_to_row_major(stream, sizeof(T) == 8 ? 1 : 0, B, ldb, workspace, cols, n);
+        if (e != 0) return e;
         a.B = (const T*)workspace; b_row_major = 1; ldb = n;
     }
     a.sbk = b_row_major ? ldb : 1; a.sbj = b_row_major ? 1 : ldb;

@@ -266,8 +266,7 @@ static void launch_csr16_v(cudaStream_t st, const dim3& grid, const SpmmCsr16Arg
 template <typename T>
 static int launch_csr16(cudaStream_t st, SpmmCsr16Args a, const Scalars<float>& sc, bool c_row, int64_t k, void* copy) {
     if (copy) {                                        // op(B)(k, j) = B[k + j * sbj]: the row-major copy, ld = n
-        const dim3 tg((unsigned)((k + 31) / 32), (unsigned)((a.n + 31) / 32));
-        spmm_transpose_b_kernel<T><<<tg, 256, 0, st>>>((const T*)a.B, a.sbj, (T*)copy, (int)k, a.n);
+        spmm_transpose_b_kernel<T><<<spmm_transpose_b_grid(k, a.n), 256, 0, st>>>((const T*)a.B, a.sbj, (T*)copy, (int)k, a.n);
         a.B = copy; a.sbk = a.n; a.sbj = 1;
     }
     const int v = csr16_v(a.n), lw = csr16_path(a.n, a.B, a.sbk, a.sbj);

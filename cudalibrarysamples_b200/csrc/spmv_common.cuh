@@ -117,22 +117,33 @@ __device__ __forceinline__ T axpby(T alpha, T sum, T beta, const T* y) {
 
 // B (cols x n, column-major, leading dimension ldb) -> Bt (cols x n, row-major, tight): 32 x 32 tiles through shared memory.
 // The row-major copy of a column-major B that spmm_csr.cu (fp32 / fp64) and spmm_csr16.cu (fp16 / bf16) read from the workspace.
+// grid.y is capped at 65535 (spmm_transpose_b_grid): a CTA walks the 32-column strips j0, j0 + 32 * gridDim.y, ... so that
+// every n up to INT32_MAX - 64 is served, not only n <= 32 * 65535.
 template <typename T>
 __global__ void __launch_bounds__(256) spmm_transpose_b_kernel(const T* __restrict__ B, long long ldb, T* __restrict__ Bt, int cols, int n) {
     __shared__ T tile[32][33];
     const int tx = (int)threadIdx.x & 31, ty = (int)threadIdx.x >> 5;
-    const int k0 = blockIdx.x * 32, j0 = blockIdx.y * 32;
+    const int k0 = blockIdx.x * 32;
+    for (long long j0 = (long long)blockIdx.y * 32; j0 < n; j0 += 32LL * gridDim.y) {      // block-uniform
 #pragma unroll
-    for (int i = 0; i < 32; i += 8) {
-        const int k = k0 + tx, j = j0 + ty + i;
-        if (k < cols && j < n) tile[ty + i][tx] = B[(long long)j * ldb + k];
-    }
-    __syncthreads();
+        for (int i = 0; i < 32; i += 8) {
+            const int k = k0 + tx;
+            const long long j = j0 + ty + i;
+            if (k < cols && j < n) tile[ty + i][tx] = B[j * ldb + k];
+        }
+        __syncthreads();
 #pragma unroll
-    for (int i = 0; i < 32; i += 8) {
-        const int k = k0 + ty + i, j = j0 + tx;
-        if (k < cols && j < n) Bt[(long long)k * n + j] = tile[tx][ty + i];
+        for (int i = 0; i < 32; i += 8) {
+            const int k = k0 + ty + i;
+            const long long j = j0 + tx;
+            if (k < cols && j < n) Bt[(long long)k * n + j] = tile[tx][ty + i];
+        }
+        __syncthreads();                                       // the tile is refilled by the next strip
     }
+}
+inline dim3 spmm_transpose_b_grid(long long cols, long long n) {
+    const long long strips = (n + 31) / 32;
+    return dim3((unsigned)((cols + 31) / 32), (unsigned)(strips < 65535 ? (strips > 0 ? strips : 1) : 65535));
 }
 
 template <typename T>

@@ -65,7 +65,7 @@ csr_short_kernel(const ShortArgs<T> a) {
     const int lane = (int)threadIdx.x & 31, warp = (int)threadIdx.x >> 5;
     T* sp = sprod[warp];
     const T alpha = a.s.a(), beta = a.s.b();
-    const int nblocks = (a.rows + 31) >> 5;
+    const int nblocks = (int)(((long long)a.rows + 31) >> 5);                    // no int overflow for rows near INT32_MAX
     for (int blk = blockIdx.x * SHORT_WARPS + warp; blk < nblocks; blk += gridDim.x * SHORT_WARPS) {   // warp-uniform
         const int row = (blk << 5) + lane;
         const bool live = row < a.rows;
