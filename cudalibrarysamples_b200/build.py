@@ -20,7 +20,7 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libb200spmv.so")
 GEN_LIB_PATH = os.path.join(PKG_DIR, "libb200gen.so")
 SPSV_LIB_PATH = os.path.join(PKG_DIR, "libb200spsv.so")
-SOURCES = ["spmv_csr.cu", "spmv_csr_flat.cu", "spmv_csr_short.cu", "spmv_csr16.cu", "spmv_csr_z.cu", "spmv_csr_transpose.cu", "spmv_coo_sell.cu", "spmv_generic.cu", "spmm_csr.cu", "spmm_coo.cu", "spmm_bell.cu", "spmm_bsr.cu", "spmm_csr16.cu", "spmm_csr_t.cu", "convert.cu", "dense_convert.cu", "batched_banded.cu", "ilu0_csr.cu", "sddmm_csr.cu", "sddmm_bsr.cu", "spsm_csr.cu", "cg_fused.cu", "bicgstab_fused.cu", "peer_sync.cu", "config.cpp", "cusparse_shim.cpp", "real_cusparse.cpp"]
+SOURCES = ["spmv_csr.cu", "spmv_csr_flat.cu", "spmv_csr_short.cu", "spmv_csr16.cu", "spmv_csr_z.cu", "spmv_csr_transpose.cu", "spmv_coo_sell.cu", "spmv_generic.cu", "spmm_csr.cu", "spmm_coo.cu", "spmm_bell.cu", "spmm_bsr.cu", "spmm_csr16.cu", "spmm_csr_t.cu", "convert.cu", "dense_convert.cu", "batched_banded.cu", "ilu0_csr.cu", "spgemm_csr.cu", "sddmm_csr.cu", "sddmm_bsr.cu", "spsm_csr.cu", "cg_fused.cu", "bicgstab_fused.cu", "peer_sync.cu", "config.cpp", "cusparse_shim.cpp", "real_cusparse.cpp"]
 GEN_SOURCES = ["workload_gen.cu"]
 SPSV_SOURCES = ["spsv_csr.cu", "spsv_shim.cpp", "real_cusparse.cpp"]
 HEADERS = ["spmv_common.cuh", "cg_reduce.cuh", "radix_sort.cuh", "csr_chunk_walk.cuh", "mma_sm90.cuh", "spsv_plan.cuh", "spmv_generic_kernels.cuh", "batched_banded.cuh", "config.h", "real_cusparse.h", os.path.join("..", "..", "include", "b200spmv.h"),

@@ -79,6 +79,12 @@ static int apply(Config& c, const char* key, const char* value) {
         else return -1;
         return 0;
     }
+    if (!strcmp(key, "B200SPMV_SPGEMM")) {
+        if (!value || !value[0] || !strcmp(value, "auto")) c.spgemm = 0;
+        else if (!strcmp(value, "on")) c.spgemm = 1;
+        else return -1;
+        return 0;
+    }
     return -1;
 }
 
@@ -88,7 +94,7 @@ Config& config() {
     std::call_once(once, [] {
         static const char* keys[] = {"B200SPMV_CSR_KERNEL", "B200SPMV_COO_KERNEL", "B200SPMV_TILE_ORDER", "B200SPMV_PDL",
                                      "B200SPMV_SEG_DENSE", "B200SPMV_SELL_GENERIC", "B200SPMV_FLAT", "B200SPMV_FLAT_QUIET", "B200SPMV_SHORT", "B200SPMV_GENERIC",
-                                     "B200SPMV_ZCSR", "B200SPMV_DENSE", "B200SPMV_BANDED", "B200SPMV_ILU0"};
+                                     "B200SPMV_ZCSR", "B200SPMV_DENSE", "B200SPMV_BANDED", "B200SPMV_ILU0", "B200SPMV_SPGEMM"};
         for (const char* k : keys)
             if (const char* v = getenv(k)) apply(c, k, v);
     });

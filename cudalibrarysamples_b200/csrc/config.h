@@ -31,6 +31,8 @@ struct Config {
                             //   call b200banded_route admits
     int ilu0        = 0;    // B200SPMV_ILU0 = auto|on: cusparse<t>csrilu02 / csric02.  auto (0, default): the native factorization only
                             //   in the classes measured at least at parity (DESIGN.md 3.26); on (1): every call b200ilu0_route admits
+    int spgemm      = 0;    // B200SPMV_SPGEMM = auto|on: cusparseSpGEMMreuse_compute.  auto (0, default): the native numeric phase only
+                            //   in the classes measured at least at parity (DESIGN.md 3.28); on (1): every call b200spgemm_route admits
 };
 
 Config& config();

@@ -595,8 +595,8 @@ B200SPMV_EXPORT int b200spmv_sell_generic_mv(void* stream, int off64, int col64,
  *                      COO, Sliced-ELL and strided-batch SpMM, which have not had their first hardware run yet)
  *   B200SPMV_ZCSR = auto|on (cusparseSpMV on a double-complex CSR A: auto [default] = b200spmv_csr_z only in the classes measured at
  *                      least at parity with the closed library (none today, DESIGN.md 3.21); on = every call in its class)
- *   B200SPMV_DENSE / B200SPMV_BANDED / B200SPMV_ILU0 = auto|on (the same choice for the conversions, the batched banded solves and
- *                      cusparse<t>csrilu02 / csric02)
+ *   B200SPMV_DENSE / B200SPMV_BANDED / B200SPMV_ILU0 / B200SPMV_SPGEMM = auto|on (the same choice for the conversions, the batched
+ *                      banded solves, cusparse<t>csrilu02 / csric02 and cusparseSpGEMMreuse_compute)
  * returns 0, or -1 for an unknown key / value. */
 B200SPMV_EXPORT int  b200spmv_set_option(const char* key, const char* value);
 /* Call counters of the cuSPARSE-symbol layer: SpMV calls that ran on our kernels, SpMV calls handed to the closed library
@@ -809,6 +809,53 @@ B200SPMV_EXPORT void b200ilu0_params(int32_t* threads_per_cta, int32_t* ctas_per
  * CUDA_R_32F / CUDA_R_64F, sizes outside int32, and every class not measured at least at parity with the closed library
  * (DESIGN.md 3.26).  B200SPMV_ILU0=on makes every call this admits native.  Host logic only. */
 B200SPMV_EXPORT int b200ilu0_route(int kind, int vtype, int64_t rows, int64_t nnz, int64_t levels);
+/* ---------------------------------------------------------------------------------------------- *
+ * Sparse x sparse, numeric phase with structure reuse (cusparseSpGEMMreuse_compute;               *
+ * cuSPARSE/spgemm_reuse), spgemm_csr.cu:                                                          *
+ *   C = alpha A B + beta C on C's stored pattern, A rows x krows, B krows x cols, C rows x cols,  *
+ *   all CSR with int32 offsets and columns, each with its own index base (0 or 1).  C's columns   *
+ *   must be strictly ascending in every row; A's and B's need not be sorted, but a B row holds a  *
+ *   column once.  dtype 0 = fp32, 1 = fp64 (values, alpha, beta, arithmetic).  Every C(i, j) is   *
+ *   acc = fadd(acc, fmul(a_ik, b_kj)) from acc = +0 over A row i in stored order, then            *
+ *   fadd(fmul(alpha, acc), fmul(beta, c_ij)), each correctly rounded (no FMA); at beta = 0 C is   *
+ *   not read and the result is fmul(alpha, acc) (DESIGN.md 3.28).  The bits depend on nothing     *
+ *   else.  A product whose column C's row does not store is skipped and counted in the plan.      *
+ *   return: 0, -1 on invalid arguments (checked before any CUDA call), else the cudaError_t.      *
+ * ---------------------------------------------------------------------------------------------- */
+#define B200SPGEMM_BAD_PATTERN (-2)     /* plan: offsets outside [0, nnz] or decreasing, C columns not strictly ascending or outside
+                                           [0, cols), A columns outside [0, krows), or a B row A names with bad offsets */
+/* Bytes of the plan: a 256-byte header (64-bit words: [0] the bad-pattern bits, [1] products compute skipped because C's row does
+ * not store their column, summed over every compute since the plan, [2] the compute kernel's pass queue, [3] the number of passes),
+ * then each row's pass count and bin and the pass list.  A closed form of the sizes (nnz_a and nnz_b do not enter it today). */
+B200SPMV_EXPORT size_t b200spgemm_plan_size(int64_t rows, int64_t nnz_a, int64_t nnz_b, int64_t nnz_c);
+/* The C columns one warp stages in shared memory (a C row longer than this is cut into windows, each re-walking A's row), the
+ * warps per CTA, and the three products-per-row edges of the four bins, heaviest first: bin b holds the rows with at least
+ * bin_edges[b] products (bin 3: the rest).  Pure. */
+B200SPMV_EXPORT void b200spgemm_params(int32_t* window, int32_t* warps_per_cta, int64_t* bin_edges /* [3] */);
+/* Builds the plan from the three patterns (values are not read): checks them on the device, counts each C row's products
+ * (int64), bins the rows and lists their windows heaviest bin first.  Synchronises the stream once, to read back the verdict:
+ * B200SPGEMM_BAD_PATTERN (and the bits in *bad) when a pattern fails, else 0 with the pass count in *passes.  Nothing outside the
+ * checked ranges is read. */
+B200SPMV_EXPORT int b200spgemm_plan(void* stream, int64_t rows, int64_t krows, int64_t cols, int64_t nnz_a, int64_t nnz_b, int64_t nnz_c,
+                                    const void* a_off, const void* a_col, int32_t a_base, const void* b_off, int32_t b_base,
+                                    const void* c_off, const void* c_col, int32_t c_base, void* plan, size_t plan_bytes, int64_t* passes,
+                                    uint64_t* bad);
+/* C's values from the plan b200spgemm_plan built for these patterns (it must have returned 0).  alpha and beta are host pointers,
+ * or device pointers read by the kernel (scalars_on_device = 1).  One memset and one launch: no allocation, no host
+ * synchronisation, CUDA-graph capturable; two computes on one plan must not overlap. */
+B200SPMV_EXPORT int b200spgemm_compute(void* stream, int dtype, int64_t rows, int64_t nnz_c, const void* a_off, const void* a_col,
+                                       const void* a_val, int32_t a_base, const void* b_off, const void* b_col, const void* b_val,
+                                       int32_t b_base, const void* c_off, const void* c_col, void* c_val, int32_t c_base,
+                                       const void* alpha, const void* beta, int scalars_on_device, void* plan);
+/* Where the shim sends cusparseSpGEMMreuse_copy's plan and cusparseSpGEMMreuse_compute (enum values as int; idx_*: the operand's
+ * cusparseIndexType_t when its offsets and columns share it, else -1): 1 = b200spgemm_compute, 0 = the closed library.  Native
+ * needs opA = opB = NON_TRANSPOSE, alg DEFAULT / CSR_ALG_DETERMINITIC / CSR_ALG_NONDETERMINITIC, three CSR operands with int32
+ * indices and bases 0 / 1, A, B, C and the compute type all CUDA_R_32F or all CUDA_R_64F, every size below 2^31 - 1, no
+ * B200SPMV_FORWARD=1, and a class measured at least at parity with the closed library (DESIGN.md 3.28: none today).
+ * B200SPMV_SPGEMM=on makes every call this admits native.  Host logic only. */
+B200SPMV_EXPORT int b200spgemm_route(int opA, int opB, int alg, int compute_type, int format_a, int format_b, int format_c, int vtype_a,
+                                     int vtype_b, int vtype_c, int idx_a, int idx_b, int idx_c, int base_a, int base_b, int base_c,
+                                     int64_t rows, int64_t krows, int64_t cols, int64_t nnz_a, int64_t nnz_b, int64_t nnz_c);
 /* name of the main kernel the most recent CSR SpMV launched, e.g. "b200::csr_seg_kernel<double>" (bench.py's roofline.kernel) */
 B200SPMV_EXPORT const char* b200spmv_last_csr_kernel(void);
 
@@ -1057,6 +1104,17 @@ B200SPMV_EXPORT cusparseStatus_t cusparseCcsric02(cusparseHandle_t, int, int, co
                                                   const int*, csric02Info_t, cusparseSolvePolicy_t, void*);
 B200SPMV_EXPORT cusparseStatus_t cusparseZcsric02(cusparseHandle_t, int, int, const cusparseMatDescr_t, cuDoubleComplex*, const int*,
                                                   const int*, csric02Info_t, cusparseSolvePolicy_t, void*);
+/* cusparse.h:5917-5920, 6019-6041 -- spgemm_reuse_example.c.  The descriptor stays the closed library's; the shim keeps a side-table
+ * entry per descriptor.  cusparseSpGEMMreuse_workEstimation / _nnz and the whole non-reuse SpGEMM API are not exported: they bind
+ * to the closed library. */
+B200SPMV_EXPORT cusparseStatus_t cusparseSpGEMM_createDescr(cusparseSpGEMMDescr_t*);
+B200SPMV_EXPORT cusparseStatus_t cusparseSpGEMM_destroyDescr(cusparseSpGEMMDescr_t);
+B200SPMV_EXPORT cusparseStatus_t cusparseSpGEMMreuse_copy(cusparseHandle_t, cusparseOperation_t, cusparseOperation_t, cusparseConstSpMatDescr_t,
+                                                          cusparseConstSpMatDescr_t, cusparseSpMatDescr_t, cusparseSpGEMMAlg_t,
+                                                          cusparseSpGEMMDescr_t, size_t*, void*);
+B200SPMV_EXPORT cusparseStatus_t cusparseSpGEMMreuse_compute(cusparseHandle_t, cusparseOperation_t, cusparseOperation_t, const void*,
+                                                             cusparseConstSpMatDescr_t, cusparseConstSpMatDescr_t, const void*,
+                                                             cusparseSpMatDescr_t, cudaDataType, cusparseSpGEMMAlg_t, cusparseSpGEMMDescr_t);
 #ifdef __cplusplus
 }
 #endif
