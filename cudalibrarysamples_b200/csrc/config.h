@@ -17,8 +17,8 @@ struct Config {
     int generic     = 1;    // B200SPMV_GENERIC = off|csr|all: what spmv_generic.cu serves instead of the closed library.
                             //   csr (default): CSR with 64-bit indices / fp32 A with fp64 vectors / their transposes / no buffer --
                             //                  validated on the GPU by tests/test_generic_gpu.py;
-                            //   all: also COO and Sliced-ELL of those kinds, Sliced-ELL transposes, strided-batch SpMM -- written
-                            //        and emulated on the CPU, their first hardware run is tests/test_zz_unverified_gpu.py;
+                            //   all: also COO and Sliced-ELL of those kinds, Sliced-ELL transposes, strided-batch SpMM -- validated
+                            //        on the GPU by tests/test_generic_opt_in_gpu.py, opt-in because unmeasured;
                             //   off: everything of that kind goes to the closed library
     int zcsr        = 0;    // B200SPMV_ZCSR = auto|on: cusparseSpMV on a double-complex CSR A.  auto (0, default): b200spmv_csr_z
                             //   only in the classes measured at least at parity (none today, DESIGN.md 3.21); on (1): every call

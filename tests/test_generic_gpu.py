@@ -4,7 +4,7 @@ Every case goes through the C ABI (the cusparse* symbols of libb200spmv.so), is 
 the same inputs and against the closed library on the same device buffers, and must be served by OUR kernels
 (b200spmv_get_stats: forwarded unchanged).  A combination the closed library itself refuses must be refused by the shim
 with the same status (cusparseSpMV_bufferSize keeps the real library's verdict).
-The COO / Sliced-ELL kernels of the same file and the strided-batch SpMM are in tests/test_zz_unverified_gpu.py.
+The COO / Sliced-ELL kernels of the same file and the strided-batch SpMM are in tests/test_generic_opt_in_gpu.py.
 
 Tolerances: fp64 arithmetic 1e-12, fp32 arithmetic 1e-5 (relative 2-norm), as in test_parity_gpu.py.
 """

@@ -387,6 +387,38 @@ def test_strided_batches_at_65535(N, dt):
     brow = [r for r in range(3) for _ in range(B_OFF[r], B_OFF[r + 1])]
     want = torch.stack([P[:, br * BS:(br + 1) * BS, bc * BS:(bc + 1) * BS] for br, bc in zip(brow, B_COL)], dim=1)
     exact(cv.view(BATCH, bnnz, BS, BS), want)
+
+
+@pytest.mark.parametrize("dt", [0, 1])
+def test_strided_batch_csr_spmm_at_65535(N, cs, api, dt):
+    """cusparseSpMM on a CSR A with a strided batch of 65535 tiny products (B200SPMV_GENERIC=all: the shim's loop of one
+    b200spmm_csr_ws per matrix): A_b's columns and values strided, offsets shared, B_b column-major (copied row-major in the buffer
+    by every product), C_b column-major, beta = 0 into NaN.  Each matrix holds other values, so a batch offset that wraps, stops
+    early or reads another product's copy of B shows."""
+    guard("strided CSR SpMM batch", 64 << 20)
+    off, col, _ = a_matrix(0)
+    nnz = A_OFF[-1]
+    row = torch.searchsorted(off, torch.arange(nnz, device="cuda"), right=True) - 1
+    V = batched((nnz,), 9)
+    Adense = torch.zeros(BATCH, A_ROWS, A_COLS, dtype=torch.int64, device="cuda")
+    Adense[:, row, col] = V
+    Bc = batched((A_COLS, N_B), 10)
+    Bs = as_dt(Bc.transpose(1, 2).reshape(-1), dt)
+    C0 = torch.full((BATCH * A_ROWS * N_B,), float("nan"), dtype=TD[dt], device="cuda")
+    arrays = dict(off=off.int(), col=col.int().repeat(BATCH), val=as_dt(V.reshape(-1), dt), nnz=nnz)
+    api.set_option("B200SPMV_GENERIC", "all")
+    try:
+        before = api.stats()
+        Cb = cs.spmm(api, A_ROWS, A_COLS, arrays, Bs, C0, LM.ALPHA, 0.0, n=N_B, alg=cs.CUSPARSE_SPMM_CSR_ALG2, batches=BATCH,
+                     colval_stride=nnz, compute=cs._VT[TD[dt]], preprocess=False)
+        torch.cuda.synchronize()
+        after = api.stats()
+    finally:
+        api.set_option("B200SPMV_GENERIC", "csr")
+    assert after["native"] == before["native"] + 1 and after["forwarded"] == before["forwarded"]
+    exact(Cb.view(BATCH, N_B, A_ROWS).transpose(1, 2), LM.ALPHA * bmm(Adense, Bc))
+    del Cb, C0, Bs, arrays
+    release(f"csr spmm batch dt={dt}")
     release(f"strided batches dt={dt}")
 
 
